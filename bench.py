@@ -1,10 +1,11 @@
 #!/usr/bin/env python
 """bench.py — env-steps/s of the A1 hot path (BASELINE.json configs[1]: 4096 parallel A1 envs, flat terrain, fixed
-ETG + random residual policy rollout) on N B200s of one node, with the roofline of the dominant kernel and the CPU
+ETG + random residual policy rollout) on N H100s of one node, with the roofline of the dominant kernel and the CPU
 oracle timed beside it.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]              # torchrun launches one rank per GPU for N>1
   python bench.py --impl reference [--gpus N] [--steps K] ...      # the CPU arm (oracle port; pybullet is absent)
+  python bench.py ... --dump-outputs DIR                           # also write the last timed step's outputs as DIR/<name>.npy
 
 A "step" is one env.step() over the whole env batch of a rank (= 13 fused physics substeps + ETG + obs/reward pack in
 ONE kernel launch).  Weak scaling: every rank owns its own 4096 envs, no data-path collective.
@@ -28,6 +29,18 @@ WORKLOAD = "BASELINE configs[1]: 4096 parallel A1 envs per GPU, flat terrain, fi
 ALG_BYTES_IN = 21 * 16 + 15 * 16 + 16 * 16 + 48 + 4 + 2 * 3 * 4 * 16      # state, params, ETG, action, counter, history reads
 ALG_BYTES_OUT = 21 * 16 + 2 * 3 * 4 * 16 + 49 * 4 + 4 + 1 + 56 * 4 + 4      # state, history writes, obs, reward, done, info, counter
 ALG_BYTES_PER_ENV_STEP = ALG_BYTES_IN + ALG_BYTES_OUT
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes {name: tensor} as out_dir/<name>.npy (float32): what a caller of the timed path received from its last step.  The inputs
+    are seeded, so two builds run with the same arguments can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        total += a.nbytes
+        assert total <= 64 * 1024 * 1024, "dump exceeds 64 MB"
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def etg_weights():
@@ -306,6 +319,8 @@ def main():
     ap.add_argument("--envs", type=int, default=ENVS_PER_GPU)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the BASELINE configs[2..4] / strong-scaling block")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write obs / reward / done / info of the last timed step (rank 0) as DIR/<name>.npy in float32")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -326,7 +341,7 @@ def main():
     # residual actions: uniform(-0.3, 0.3), counter-based per (seed, rank, step) pool resident in HBM
     g = torch.Generator(device=dev); g.manual_seed(1234 + rank)
     pool = torch.rand(64, n, 12, device=dev, generator=g) * 0.6 - 0.3
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev, dtype=torch.float32)     # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev, dtype=torch.float32)     # > 50 MB L2
     for k in range(W):
         env.step(pool[k % 64])
     torch.cuda.synchronize()
@@ -347,6 +362,7 @@ def main():
     if world > 1:
         dist.barrier()
     launches = env.launch_count() - l0
+    last = {k: v.clone() for k, v in zip(("obs", "reward", "done", "info"), (env.obs, env.reward, env.done, env.info))} if args.dump_outputs else None
     total_ms = sum(a.elapsed_time(bb) for a, bb in ev)
     t = torch.tensor([total_ms], device=dev, dtype=torch.float64)
     if world > 1:
@@ -395,28 +411,11 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak_gbs, peak_src = (peaks.get("hbm_gbs"), "measured (MEASURED_PEAKS.json hbm_gbs)") if peaks.get("hbm_gbs") else (6650.0, "fallback")
+        peak_gbs, peak_src = (peaks.get("hbm_gbs"), "measured (MEASURED_PEAKS.json hbm_gbs)") if peaks.get("hbm_gbs") else (3350.0, "H100 SXM data sheet")
         ms_per_step = total_ms / K
         achieved = ALG_BYTES_PER_ENV_STEP * n / (ms_per_step * 1e-3) / 1e9
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "step_kernel_traffic.json"))).get("dram_bytes_per_launch")
-        except Exception:
-            pass
-        # secondary (the bound that actually applies, SURVEY §8d): warp-instruction issue slots.  Instructions per launch are the
-        # ncu count of the committed capture (profiles/step_kernel_r01e_ncu_full.csv); duration and SM clock are this run's.
-        issue = None
-        try:
-            cands = sorted(f for f in os.listdir(os.path.join(ROOT, "profiles")) if f.startswith("step_kernel_r0") and f.endswith("_ncu_full.csv"))
-            prof_name = cands[-1]
-            prof = dict(l.split(",")[0::2] for l in open(os.path.join(ROOT, "profiles", prof_name)).read().splitlines()[2:] if l.count(",") == 2)
-            inst = float(prof["smsp__inst_executed.sum"]) * n / 4096.0
-            mhz = (clocks or {}).get("sm_mhz") or 1965.0
-            slots = ms_per_step * 1e-3 * mhz * 1e6 * 148 * 4
-            issue = {"warp_instructions_per_launch": inst, "issue_slot_frac": inst / slots, "fma_pipe_pct_ncu": float(prof["sm__pipe_fma_cycles_active.avg.pct_of_peak_sustained_active"]),
-                     "warps_per_sm_ncu": float(prof["sm__warps_active.avg.per_cycle_active"]), "source": "profiles/" + prof_name}
-        except Exception:
-            pass
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last)
         cpu = None
         if not args.no_cpu_baseline:
             threads = host_threads()
@@ -435,8 +434,9 @@ def main():
             "e2e": {"value": e2e_val, "unit": "env-steps/s", "h2d_bytes_per_step": env.h2d_bytes_per_step(), "d2h_bytes_per_step": env.d2h_bytes_per_step(info=True), "steps": Ke, "estimator": "median of %d blocks of %d steps (wall clock)" % (NBLK, blk), "block_rates_rank0": e2e_blocks,
                     "transport": "numpy action -> pinned buffer -> step kernel reads it over PCIe and stores obs|reward|done and the info rows [N,56] (staged in shared memory, one coalesced block per CTA) straight to pinned host memory (b2q_step_host, B2Q_HOST_IO=2); stream sync every step"},
             "gpu_launches": int(launches),
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s", "frac": achieved / peak_gbs, "traffic": traffic,
-                         "peak_source": peak_src, "kernel": "b2q_step_kernel<float>", "alg_bytes_per_env_step": ALG_BYTES_PER_ENV_STEP, "issue": issue,
+            "gpu": {"name": torch.cuda.get_device_name(dev), "sms": torch.cuda.get_device_properties(dev).multi_processor_count},
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s", "frac": achieved / peak_gbs,
+                         "peak_source": peak_src, "kernel": "b2q_step_kernel<float>", "alg_bytes_per_env_step": ALG_BYTES_PER_ENV_STEP,
                          "note": "latency/FP32-issue bound by construction (13 substeps x 23 PGS sweeps per launch on ~2.4 KB of state): HBM fraction is structurally tiny, see DESIGN.md §5"},
             "cpu_baseline": cpu,
             "clocks": clocks,

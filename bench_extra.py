@@ -31,7 +31,7 @@ def main():
     from paddlerobotics_b200.es import PopulationEvaluator
     w, b = etg_weights()
     out = []
-    # config 2 with the policy in the loop: obs -> fused MLP (tcgen05) -> env.step, 4096 envs
+    # config 2 with the policy in the loop: obs -> fused MLP (wgmma) -> env.step, 4096 envs
     env = VecQuadrupedalEnv(4096, auto_reset=True); env.reset(w, b)
     ag = MujocoAgent(49, 12, seed=0)
     state = {"obs": env.obs}
@@ -41,10 +41,10 @@ def main():
     out.append({"what": "rollout 4096 envs, policy in the loop (fused MLP + step kernel)", "ms_per_step": ms, "env_steps_per_s": 4096 / ms * 1e3})
     obs = torch.randn(4096, 49, device="cuda")
     ms = timed(lambda: ag.actor.forward(obs), 300, 20)
-    out.append({"what": "actor MLP forward M=4096 (tcgen05)", "ms": ms, "tflops": 2 * 4096 * (64 * 256 + 256 * 256 + 256 * 32) / ms / 1e9})
+    out.append({"what": "actor MLP forward M=4096 (wgmma)", "ms": ms, "tflops": 2 * 4096 * (64 * 256 + 256 * 256 + 256 * 32) / ms / 1e9})
     obs8 = torch.randn(8192, 49, device="cuda")
     ms = timed(lambda: ag.actor.forward(obs8), 300, 20)
-    out.append({"what": "actor MLP forward M=8192 (tcgen05)", "ms": ms})
+    out.append({"what": "actor MLP forward M=8192 (wgmma)", "ms": ms})
     env.close()
     # config 4: SAC update, batch 8192 (and the reference's 256)
     for B in (256, 8192):

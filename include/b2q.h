@@ -1,4 +1,4 @@
-/* b2q.h — C ABI of the B200-native batched A1 simulator + rollout engine (libb2q.so).
+/* b2q.h — C ABI of the H100-native batched A1 simulator + rollout engine (libb2q.so).
  *
  * This is the drop-in boundary for the ONE hot path of PaddleRobotics QuadrupedalRobots/ETGRL: everything
  * below `env.reset / env.step` (and, for the policy, below `agent.predict / agent.sample`).  Plain C types

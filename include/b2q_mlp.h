@@ -1,5 +1,5 @@
-/* b2q_mlp.h — C ABI of the fused 3-layer policy/critic MLP forward (K3) on 5th-gen tensor cores (tcgen05 + TMEM,
- * operands staged in shared memory by bulk async copies / TMA).  Device pointers, caller's stream, 0 on success.
+/* b2q_mlp.h — C ABI of the fused 3-layer policy/critic MLP forward (K3) on Hopper tensor cores (wgmma,
+ * operands staged in shared memory by bulk async copies).  Device pointers, caller's stream, 0 on success.
  *
  * Reference interfaces replaced (QuadrupedalRobots/ETGRL):
  *   Actor.forward   obs -> relu(l1) -> relu(l2) -> {mean_linear, std_linear}, clamp log_std   model/mujoco_model.py:44-60

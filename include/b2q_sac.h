@@ -1,4 +1,4 @@
-/* b2q_sac.h — C ABI of the SAC learner step (K5/K6): critic + actor losses, backward passes on tcgen05 tensor cores,
+/* b2q_sac.h — C ABI of the SAC learner step (K5/K6): critic + actor losses, backward passes on wgmma tensor cores,
  * Adam, Polyak target sync — all on the device.  Device pointers, caller's stream, 0 on success.
  *
  * Reference interfaces replaced (QuadrupedalRobots/ETGRL):

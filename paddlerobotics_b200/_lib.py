@@ -32,7 +32,7 @@ SYMBOLS = {
     "b2q_set_state": (_i, [_vp, _vp, _vp]),
     "b2q_get_step_count": (_i, [_vp, _vp, _vp]),
     "b2q_launch_count": (C.c_int64, [_vp]),
-    # policy / critic MLP forward on tcgen05 — include/b2q_mlp.h
+    # policy / critic MLP forward on wgmma tensor cores — include/b2q_mlp.h
     "b2q_mlp_create": (_i, [_i, _i, _i, _i, C.POINTER(_vp)]),
     "b2q_mlp_destroy": (_i, [_vp]),
     "b2q_mlp_last_error": (C.c_char_p, [_vp]),
@@ -80,7 +80,7 @@ def load():
     if not os.path.exists(_LIB_PATH):
         raise RuntimeError(
             "paddlerobotics_b200: %s is missing — build it with `python -m paddlerobotics_b200.build` "
-            "(nvcc, sm_100a). There is no CPU/PyTorch fallback for this path." % _LIB_PATH)
+            "(nvcc, sm_90a). There is no CPU/PyTorch fallback for this path." % _LIB_PATH)
     lib = C.CDLL(_LIB_PATH)
     for name, (res, args) in SYMBOLS.items():
         fn = getattr(lib, name)  # AttributeError if the ABI is incomplete

@@ -1,5 +1,5 @@
 """PARL-surface agent (`MujocoAgent.predict / sample / restore / save`, ETGRL/model/mujoco_agent.py:20-65) on top of the
-fused tcgen05 MLP kernel (csrc/b2q_mlp.cu).  Parameters are held as float32 torch tensors under the reference's
+fused wgmma MLP kernel (csrc/b2q_mlp.cu).  Parameters are held as float32 torch tensors under the reference's
 state-dict key names (`actor_model.{l1,l2,mean_linear,std_linear}.{weight,bias}`, `critic_model.l1..l6.*`, SURVEY App. A)
 so the reference's `.pt` checkpoints load unchanged; the kernel consumes bf16 images repacked on the device.
 """
@@ -21,7 +21,7 @@ class FusedMLP:
     def __init__(self, in_dim, out_dim, nets=1, device=0, borrowed=None):
         self._owned = borrowed is None
         if not torch.cuda.is_available():
-            raise RuntimeError("FusedMLP needs a CUDA device (tcgen05 kernel, no fallback)")
+            raise RuntimeError("FusedMLP needs a CUDA device (wgmma kernel, no fallback)")
         self.lib = _lib.load()
         self.in_dim, self.out_dim, self.nets = in_dim, out_dim, nets
         self.device = torch.device("cuda", int(device))

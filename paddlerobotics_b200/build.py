@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a CUDA library (csrc/libb2q.so).  nvcc cross-compiles without a GPU."""
+"""In-tree build of the sm_90a CUDA library (csrc/libb2q.so).  nvcc cross-compiles without a GPU."""
 import os
 import subprocess
 
@@ -6,7 +6,7 @@ CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 LIB = os.path.join(CSRC, "libb2q.so")
 SOURCES = ["b2q_api.cu", "b2q_mlp.cu", "b2q_es.cu", "b2q_sac.cu", "b2q_rpm.cu"]
 HEADERS = ["b2q_sim.cuh", "b2q_math.cuh", "b2q_host_common.h", "b2q_model_host.h", "b2q_tc.cuh", "../../include/b2q.h", "../../include/b2q_mlp.h", "../../include/b2q_es.h", "../../include/b2q_sac.h", "../../include/b2q_rpm.h", "b2q_mlp_internal.h"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 
 def _stale():
@@ -21,7 +21,7 @@ def _stale():
 
 
 def build(force=False, verbose=False):
-    """Compiles every CUDA source for sm_100a into csrc/libb2q.so."""
+    """Compiles every CUDA source for sm_90a into csrc/libb2q.so."""
     if not force and not _stale():
         return LIB
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]

@@ -1,4 +1,4 @@
-// b2q_api.cu — sm_100a kernels and the C ABI (include/b2q.h) of the batched A1 simulator.
+// b2q_api.cu — sm_90a kernels and the C ABI (include/b2q.h) of the batched A1 simulator.
 //
 // Kernel map (SURVEY.md §7): K1 b2q_step_kernel (hot: R fused physics substeps + ETG + obs/reward pack, optional
 // in-kernel auto-reset), K2 b2q_reset_kernel (masked snapshot copy), b2q_settle_kernel (builds the snapshot), and
@@ -414,7 +414,7 @@ struct B2QEnv { EnvBase* impl; };
 extern "C" {
 
 void b2q_default_config(B2QConfig* cfg) { if (cfg) default_config(cfg); }
-const char* b2q_version(void) { return "b2q 0.1.0 (sm_100a)"; }
+const char* b2q_version(void) { return "b2q 0.1.0 (sm_90a)"; }
 
 int b2q_create(const B2QConfig* cfg, B2QHandle* out) {
   if (!cfg || !out) { g_create_err = "null argument"; return B2Q_EINVAL; }

@@ -1,4 +1,4 @@
-// b2q_math.cuh — small fixed-size algebra used by the A1 step kernels (sm_100a) and by the host SIMT
+// b2q_math.cuh — small fixed-size algebra used by the A1 step kernels (sm_90a) and by the host SIMT
 // emulation harness in tests/emu (same source, different Comm policy).
 #pragma once
 #include <cmath>
@@ -102,15 +102,15 @@ B2Q_HD void m_sincos(float a, float& s, float& c) {
 }
 B2Q_HD void m_sincos(double a, double& s, double& c) { s = sin(a); c = cos(a); }
 
-// two-wide value for the packed FP32 FMA of sm_100 (FFMA2: two f32 FMAs per instruction on a 64-bit register pair)
+// two-wide value: the Delassus build of the f32 solver works on PAIRS of adjacent rows.  On the device every lane op is an explicitly
+// rounded intrinsic, so the compiler never contracts a multiply and an add of a pair into one FMA: the result is the same on every target.
 template <typename T>
 struct P2 {
   T x, y;
 };
 B2Q_HD P2<float> p2fma(P2<float> a, P2<float> b, P2<float> c) {
 #if defined(__CUDA_ARCH__)
-  float2 r = __ffma2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y), make_float2(c.x, c.y));
-  P2<float> o; o.x = r.x; o.y = r.y; return o;
+  P2<float> o; o.x = __fmaf_rn(a.x, b.x, c.x); o.y = __fmaf_rn(a.y, b.y, c.y); return o;
 #else
   P2<float> o; o.x = fmaf(a.x, b.x, c.x); o.y = fmaf(a.y, b.y, c.y); return o;
 #endif
@@ -118,8 +118,7 @@ B2Q_HD P2<float> p2fma(P2<float> a, P2<float> b, P2<float> c) {
 B2Q_HD P2<double> p2fma(P2<double> a, P2<double> b, P2<double> c) { P2<double> o; o.x = fma(a.x, b.x, c.x); o.y = fma(a.y, b.y, c.y); return o; }
 B2Q_HD P2<float> p2mul(P2<float> a, P2<float> b) {
 #if defined(__CUDA_ARCH__)
-  float2 r = __fmul2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y));
-  P2<float> o; o.x = r.x; o.y = r.y; return o;
+  P2<float> o; o.x = __fmul_rn(a.x, b.x); o.y = __fmul_rn(a.y, b.y); return o;
 #else
   P2<float> o; o.x = a.x * b.x; o.y = a.y * b.y; return o;
 #endif
@@ -127,14 +126,13 @@ B2Q_HD P2<float> p2mul(P2<float> a, P2<float> b) {
 B2Q_HD P2<double> p2mul(P2<double> a, P2<double> b) { P2<double> o; o.x = a.x * b.x; o.y = a.y * b.y; return o; }
 B2Q_HD P2<float> p2add(P2<float> a, P2<float> b) {
 #if defined(__CUDA_ARCH__)
-  float2 r = __fadd2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y));
-  P2<float> o; o.x = r.x; o.y = r.y; return o;
+  P2<float> o; o.x = __fadd_rn(a.x, b.x); o.y = __fadd_rn(a.y, b.y); return o;
 #else
   P2<float> o; o.x = a.x + b.x; o.y = a.y + b.y; return o;
 #endif
 }
 B2Q_HD P2<double> p2add(P2<double> a, P2<double> b) { P2<double> o; o.x = a.x + b.x; o.y = a.y + b.y; return o; }
-template <typename T> B2Q_HD P2<T> p2s(T s) { P2<T> o; o.x = s; o.y = s; return o; }   // scalar broadcast (an operand form of FFMA2, no instruction)
+template <typename T> B2Q_HD P2<T> p2s(T s) { P2<T> o; o.x = s; o.y = s; return o; }   // scalar broadcast
 template <typename T> B2Q_HD P2<T> p2mk(T x, T y) { P2<T> o; o.x = x; o.y = y; return o; }
 
 template <typename T>

@@ -1,14 +1,14 @@
-// b2q_mlp.cu — K3: fused 3-layer MLP forward (in<=64 -> 256 -> 256 -> out<=32) on tcgen05 tensor cores.
+// b2q_mlp.cu — K3: fused 3-layer MLP forward (in<=64 -> 256 -> 256 -> out<=32) on Hopper warpgroup MMAs (wgmma).
 //
-// One CTA (256 threads: two warps per TMEM lane quarter, each taking half of the columns in the epilogues) per 128-row tile of the batch:
+// One CTA (256 threads = two warpgroups, each owning 64 rows of the tile in its MMAs) per 128-row tile of the batch:
 //   * weights live in HBM as ready-made shared-memory images (bf16, K-major, 128-byte swizzle, 64-column panels) and are
-//     brought in by bulk async copies (cp.async.bulk -> UBLKCP) that complete on mbarriers;
+//     brought in by bulk async copies (cp.async.bulk) that complete on mbarriers;
 //   * the input tile is converted f32 -> bf16 by the CTA's threads straight into the swizzled A-operand layout;
-//   * each layer is a chain of tcgen05.mma (M=128, N=256|32, K=16) issued by ONE thread, accumulating in TMEM
-//     (layer 1 -> columns 0..255, layer 2 -> 256..511, layer 3 -> 0..31); tcgen05.commit signals an mbarrier;
-//   * the epilogue warps read the accumulator with tcgen05.ld (each thread owns one row = one TMEM lane), apply
-//     bias+ReLU in f32, and write the bf16 activations back into the A-operand region for the next layer, so
-//     activations never leave the SM; the last epilogue applies tanh / clamp / sampling / log-prob and stores f32.
+//   * each layer is a chain of wgmma.mma_async (M=64 per warpgroup, N=256|32, K=16) with both operands in shared memory,
+//     accumulating in registers (128 f32 per thread for N=256);
+//   * the epilogue applies bias+ReLU in f32 to the accumulator fragment and writes the bf16 activations back into the A-operand
+//     region for the next layer, so activations never leave the SM; the last epilogue applies tanh / clamp / sampling /
+//     log-prob and stores f32.
 // Shared memory: A 64 KB | W2 128 KB | W1 then W3 32 KB | biases 2.1 KB | barriers  = 226.2 KB (of 227 KB).
 // Reference: Actor/Critic.forward (model/mujoco_model.py:44-89), SAC.predict/sample (alg/sac.py:60-75).
 #include <cuda_runtime.h>
@@ -79,19 +79,20 @@ __device__ __forceinline__ float head_actions(const uint32_t (&r)[32], const flo
 constexpr int NTHR = 256;
 __global__ void __launch_bounds__(NTHR, 1) b2q_mlp_fwd_kernel(FwdArgs a) { pdl_sync();
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, net = blockIdx.y;
-  const int trow = tid & (TILE_M - 1), chalf = tid >> 7;   // tile row owned in the epilogues; column half (0: cols 0..127, 1: 128..255)
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, net = blockIdx.y;
+  const int trow = tid & (TILE_M - 1), chalf = tid >> 7;   // row-wise passes: tile row owned; column half (0: cols 0..127, 1: 128..255)
+  const int wg = tid >> 7;                                 // warpgroup: MMA rows 64 wg .. 64 wg + 63 of the tile
+  const int fr0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), fc0 = 2 * (lane & 3);   // accumulator fragment: rows fr0, fr0 + 8; columns 8 j + fc0 + {0, 1}
   const int row0 = blockIdx.x * TILE_M, row = row0 + trow;
   const uint32_t sbase = smem_u32(smem);
   if ((sbase & 1023u) != 0) __trap();   // SWIZZLE_128B operands need a 1024-byte aligned base
-  const uint32_t sA = sbase + OFF_A, sW2 = sbase + OFF_W2, sW13 = sbase + OFF_W13;
-  const uint32_t bar_w1 = sbase + OFF_BAR, bar_w2 = bar_w1 + 8, bar_w3 = bar_w1 + 16, bar_mma = bar_w1 + 24, bar_w2t = bar_w1 + 32;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + OFF_BAR + 40);
+  const uint32_t sA = sbase + OFF_A, sAw = sA + (uint32_t)wg * 64u * 128u, sW2 = sbase + OFF_W2, sW13 = sbase + OFF_W13;
+  const uint32_t bar_w1 = sbase + OFF_BAR, bar_w2 = bar_w1 + 8, bar_w3 = bar_w1 + 16, bar_w2t = bar_w1 + 32;
   const float* bias = reinterpret_cast<const float*>(smem + OFF_BIAS);
   const uint8_t* img = a.img + (size_t)net * a.img_stride;
 
   if (tid == 0) {
-    mbar_init(bar_w1, 1); mbar_init(bar_w2, 1); mbar_init(bar_w3, 1); mbar_init(bar_mma, 1); mbar_init(bar_w2t, 1);
+    mbar_init(bar_w1, 1); mbar_init(bar_w2, 1); mbar_init(bar_w3, 1); mbar_init(bar_w2t, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     // weights: W1 (+biases) first, then W2 in 32 KB pieces
     mbar_expect_tx(bar_w1, SZ_W1 + SZ_BIAS);
@@ -100,10 +101,6 @@ __global__ void __launch_bounds__(NTHR, 1) b2q_mlp_fwd_kernel(FwdArgs a) { pdl_s
     mbar_expect_tx(bar_w2, SZ_W2);
 #pragma unroll
     for (int i = 0; i < 4; i++) bulk_g2s(sW2 + i * 32768u, img + IMG_W2 + (size_t)i * 32768u, 32768u, bar_w2);
-  }
-  if (warp == 1) {  // TMEM: all 512 columns (one CTA per SM by construction: 226 KB of shared memory)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(const_cast<const uint32_t*>(tmem_slot))), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   // input tile: f32 [rows, in_dim] (two sources concatenated) -> bf16 swizzled panel 0 (K padded to 64 with zeros)
   {
@@ -124,21 +121,16 @@ __global__ void __launch_bounds__(NTHR, 1) b2q_mlp_fwd_kernel(FwdArgs a) { pdl_s
       *reinterpret_cast<__nv_bfloat16*>(smem + OFF_A + sw128_offset((tid >> 6) + 4 * j, k, TILE_M)) = __float2bfloat16(v[j]);
   }
   fence_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t lane_addr = tmem + ((uint32_t)((warp & 3) * 32) << 16);   // a warp may touch TMEM lanes 32*(warp%4)..+31
 
   // Activation dumps for the backward pass, written from the shared-memory tile the epilogue just produced (while the next layer's MMAs
   // read the same tile): row-major [batch][256] with one full 512-byte row per warp instruction, and the [256][batch] copy as 16-byte
-  // runs of eight consecutive batch rows per column (the epilogue's own registers hold one ROW per thread: its stores would be 2-byte
-  // scatters for the transposed copy and half-used sectors for the row-major one).
+  // runs of eight consecutive batch rows per column (the accumulator fragments spread a row over four threads: their stores would be
+  // 4-byte scatters for the transposed copy and quarter-used sectors for the row-major one).
   auto dump_tile = [&](__nv_bfloat16* d_rm, __nv_bfloat16* d_t, int ncols /*256: hidden activations (per net), 64: the input tile (shared by the nets)*/) {
     const int nrows = min(TILE_M, a.M - row0);
     const size_t nbase = ncols == HID ? (size_t)net : 0;
     if (d_rm) {
-      const int lane = tid & 31;
       if (lane * 8 < ncols)
         for (int r = warp; r < nrows; r += NTHR / 32) {
           const uint4 v = *reinterpret_cast<const uint4*>(smem + OFF_A + sw128_offset(r, lane * 8, TILE_M));
@@ -166,121 +158,123 @@ __global__ void __launch_bounds__(NTHR, 1) b2q_mlp_fwd_kernel(FwdArgs a) { pdl_s
       }
     }
   };
-  // ---- layer 1: [128 x 64] x [256 x 64]^T -> TMEM cols 0..255
-  if (tid == 0) {
-    mbar_wait(bar_w1, 0);
-    tc_fence_after();
-    const uint32_t idesc = umma_idesc(TILE_M, HID);
+  // a layer over the K = 256 hidden width: 16 K-steps of 16, A = this warpgroup's 64 rows of the 4-panel tile, B = a [n_rows][256] operand image
+  float acc[128];
 #pragma unroll
-    for (int ks = 0; ks < 4; ks++) umma_f16(tmem, umma_desc(sA + ks * 32), umma_desc(sW13 + ks * 32), idesc, ks > 0);
-    umma_commit(bar_mma);
-  }
-  __syncwarp();
-  if (a.save && net == 0 && (a.sv.x_rm || a.sv.x_t)) { dump_tile(a.sv.x_rm, a.sv.x_t, 64); __syncthreads(); }   // the input tile (panel 0), before epilogue 1 overwrites it
-  mbar_wait(bar_mma, 0);
-  tc_fence_after();
-  if (tid == 0) {  // W1 is consumed: reuse its region for W3
+  for (int i = 0; i < 128; i++) acc[i] = 0.f;
+  auto mma_hidden_256 = [&](uint32_t sb) {
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 16; ks++)
+      Wgmma<HID>::mma(acc, wg_desc(sAw + (ks >> 2) * (TILE_M * 128) + (ks & 3) * 32), wg_desc(sb + (ks >> 2) * (HID * 128) + (ks & 3) * 32), ks > 0);
+    wg_commit();
+  };
+  auto mma_done = [&]() { wg_wait0(); wg_fence_acc(acc); };
+
+  // ---- layer 1: [128 x 64] x [256 x 64]^T -> acc (each warpgroup its 64 rows)
+  mbar_wait(bar_w1, 0);
+  wg_fence();
+#pragma unroll
+  for (int ks = 0; ks < 4; ks++) Wgmma<HID>::mma(acc, wg_desc(sAw + ks * 32), wg_desc(sW13 + ks * 32), ks > 0);
+  wg_commit();
+  if (a.save && net == 0 && (a.sv.x_rm || a.sv.x_t)) dump_tile(a.sv.x_rm, a.sv.x_t, 64);   // the input tile (panel 0), before epilogue 1 overwrites it
+  mma_done();
+  __syncthreads();   // both warpgroups are done with W1 and the input tile
+  if (tid == 0) {    // W1 is consumed: reuse its region for W3
     mbar_expect_tx(bar_w3, SZ_W3 + (a.da ? SZ_W1A : 0u));
     bulk_g2s(sW13, img + IMG_W3, SZ_W3, bar_w3);
     if (a.da) bulk_g2s(sW13 + OFF_W1A_IN_W13, img + IMG_W1A, SZ_W1A, bar_w3);
   }
-  // relu'(h1) of the thread's 128 columns (bit j of word cc: column 32 (4 chalf + cc) + j), kept for the input-gradient pass
+  // relu'(h1) of the thread's fragment (bit 4 j + 2 h + e of the 128: word j >> 3), kept for the input-gradient pass
   uint32_t m1[4] = {0u, 0u, 0u, 0u};
-  auto epilogue_hidden = [&](uint32_t col_base, const float* b, bool keep_mask) {
+  // bias + ReLU in f32, bf16 back into the A-operand tile for the next layer (a warpgroup writes only the rows its own MMAs read)
+  auto epilogue_hidden = [&](const float* b, bool keep_mask) {
 #pragma unroll
-    for (int c4 = 0; c4 < 4; c4++) {
-      const int cc = 4 * chalf + c4;
-      uint32_t r[32];
-      __syncwarp();
-      tmem_ld32(lane_addr + col_base + cc * 32, r);
-      uint32_t mk = 0u;
+    for (int j = 0; j < 32; j++) {
+      const int c = 8 * j + fc0;
+      const float b0 = b[c], b1 = b[c + 1];
 #pragma unroll
-      for (int j0 = 0; j0 < 32; j0 += 8) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) {
-          float v0 = fmaxf(__uint_as_float(r[j0 + j]) + b[cc * 32 + j0 + j], 0.f);
-          float v1 = fmaxf(__uint_as_float(r[j0 + j + 1]) + b[cc * 32 + j0 + j + 1], 0.f);
-          mk |= (v0 > 0.f ? 1u : 0u) << (j0 + j);
-          mk |= (v1 > 0.f ? 1u : 0u) << (j0 + j + 1);
-          __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1);
-          pk[j >> 1] = *reinterpret_cast<uint32_t*>(&h);
-        }
-        *reinterpret_cast<uint4*>(smem + OFF_A + sw128_offset(trow, cc * 32 + j0, TILE_M)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+      for (int h = 0; h < 2; h++) {
+        const float v0 = fmaxf(acc[4 * j + 2 * h] + b0, 0.f), v1 = fmaxf(acc[4 * j + 2 * h + 1] + b1, 0.f);
+        if (keep_mask) m1[j >> 3] |= ((v0 > 0.f ? 1u : 0u) | (v1 > 0.f ? 2u : 0u)) << (4 * (j & 7) + 2 * h);
+        *reinterpret_cast<__nv_bfloat162*>(smem + OFF_A + sw128_offset(fr0 + 8 * h, c, TILE_M)) = __floats2bfloat162_rn(v0, v1);
       }
-      if (keep_mask) m1[c4] = mk;
     }
   };
-  epilogue_hidden(0, bias, a.da != nullptr);
+  epilogue_hidden(bias, a.da != nullptr);
   fence_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
 
-  // ---- layer 2: [128 x 256] x [256 x 256]^T -> TMEM cols 256..511
-  if (tid == 0) {
-    mbar_wait(bar_w2, 0);
-    tc_fence_after();
-    const uint32_t idesc = umma_idesc(TILE_M, HID);
-#pragma unroll
-    for (int ks = 0; ks < 16; ks++)
-      umma_f16(tmem + 256, umma_desc(sA + (ks >> 2) * (TILE_M * 128) + (ks & 3) * 32), umma_desc(sW2 + (ks >> 2) * (HID * 128) + (ks & 3) * 32), idesc, ks > 0);
-    umma_commit(bar_mma);
-  }
-  __syncwarp();
-  if (a.save) { dump_tile(a.sv.h1_rm, a.sv.h1_t, HID); __syncthreads(); }   // reads of the h1 tile end before any thread's next epilogue overwrites it
-  mbar_wait(bar_mma, 1);
-  tc_fence_after();
+  // ---- layer 2: [128 x 256] x [256 x 256]^T -> acc
+  mbar_wait(bar_w2, 0);
+  mma_hidden_256(sW2);
+  if (a.save) dump_tile(a.sv.h1_rm, a.sv.h1_t, HID);
+  mma_done();
+  __syncthreads();   // reads of W2 and of the h1 tile end before anything overwrites them
   if (a.da && tid == 0) {   // layer 2 has consumed W2: its region takes the W2^T image for the input-gradient pass
     mbar_expect_tx(bar_w2t, SZ_W2);
 #pragma unroll
     for (int i = 0; i < 4; i++) bulk_g2s(sW2 + i * 32768u, img + IMG_W2T + (size_t)i * 32768u, 32768u, bar_w2t);
   }
-  epilogue_hidden(256, bias + HID, false);
+  epilogue_hidden(bias + HID, false);
   fence_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
 
-  // ---- layer 3: [128 x 256] x [32 x 256]^T -> TMEM cols 0..31
-  if (tid == 0) {
-    mbar_wait(bar_w3, 0);
-    tc_fence_after();
-    const uint32_t idesc = umma_idesc(TILE_M, 32);
+  // ---- layer 3: [128 x 256] x [32 x 256]^T -> acc3
+  float acc3[16];
 #pragma unroll
-    for (int ks = 0; ks < 16; ks++)
-      umma_f16(tmem, umma_desc(sA + (ks >> 2) * (TILE_M * 128) + (ks & 3) * 32), umma_desc(sW13 + (ks >> 2) * (32 * 128) + (ks & 3) * 32), idesc, ks > 0);
-    umma_commit(bar_mma);
-  }
-  __syncwarp();
+  for (int i = 0; i < 16; i++) acc3[i] = 0.f;
+  mbar_wait(bar_w3, 0);
+  wg_fence();
+#pragma unroll
+  for (int ks = 0; ks < 16; ks++)
+    Wgmma<32>::mma(acc3, wg_desc(sAw + (ks >> 2) * (TILE_M * 128) + (ks & 3) * 32), wg_desc(sW13 + (ks >> 2) * (32 * 128) + (ks & 3) * 32), ks > 0);
+  wg_commit();
   if (a.save) dump_tile(a.sv.h2_rm, a.sv.h2_t, HID);   // the head epilogue does not write the tile: no barrier needed
-  mbar_wait(bar_mma, 0);
-  tc_fence_after();
-  // Head epilogue.  RAW (critics, BC): the row's thread of column half 0 stores its outputs.  PREDICT / SAMPLE (actor): BOTH threads of a row
-  // (the two column halves read the same 32 TMEM columns) take every second action — the per-action tanh / exp / log / counter-RNG work is the
-  // longest stretch of the actor forward — and the log-prob halves meet in shared memory.  All indices are compile-time (no local arrays).
+  wg_wait0();
+  wg_fence_acc(acc3);
   {
-    uint32_t r[32];
-    __syncwarp();
-    tmem_ld32(lane_addr, r);
     const float* b3 = bias + 2 * HID;
-    float* slp = reinterpret_cast<float*>(smem + OFF_BAR + 64);            // [128] log-prob share of column half 1
-    const int od = a.out_dim, A = od >> 1;
-    const size_t orow = (size_t)net * a.M + row;
-    if (chalf == 0 && row < a.M && (a.raw || a.mode == B2Q_MLP_RAW)) {
+    const int od = a.out_dim;
+    // RAW outputs (critics, BC, the actor's raw head) straight from the fragment
+    if (a.raw || a.mode == B2Q_MLP_RAW) {
 #pragma unroll
-      for (int j = 0; j < 32; j++) {
-        if (j < od) {
-          const float y = __uint_as_float(r[j]) + b3[j];
-          if (a.raw) a.raw[orow * od + j] = y;
-          if (a.mode == B2Q_MLP_RAW) a.out[orow * od + j] = y;
-        }
-      }
+      for (int j = 0; j < 4; j++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int c = 8 * j + fc0 + e, gr = row0 + fr0 + 8 * h;
+            if (c < od && gr < a.M) {
+              const float y = acc3[4 * j + 2 * h + e] + b3[c];
+              const size_t orow = (size_t)net * a.M + gr;
+              if (a.raw) a.raw[orow * od + c] = y;
+              if (a.mode == B2Q_MLP_RAW) a.out[orow * od + c] = y;
+            }
+          }
     }
+    // PREDICT / SAMPLE (actor): the head needs a row's mean and log-std together, so the [128 x 32] result is staged row-wise in the W2
+    // region (free: the input-gradient pass, the only later reader of that region, runs for RAW critics only).  BOTH threads of a row then
+    // take every second action — the per-action tanh / exp / log / counter-RNG work is the longest stretch of the actor forward — and the
+    // log-prob halves meet in shared memory.  All register indices are compile-time (no local arrays).
     if (a.mode != B2Q_MLP_RAW) {
+      constexpr int LDS = 33;
+      float* stage = reinterpret_cast<float*>(smem + OFF_W2);
+#pragma unroll
+      for (int j = 0; j < 4; j++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) stage[(fr0 + 8 * h) * LDS + 8 * j + fc0 + e] = acc3[4 * j + 2 * h + e];
+      __syncthreads();
+      uint32_t r[32];
+#pragma unroll
+      for (int j = 0; j < 32; j++) r[j] = __float_as_uint(stage[trow * LDS + j]);
+      float* slp = reinterpret_cast<float*>(smem + OFF_BAR + 64);            // [128] log-prob share of column half 1
+      const size_t orow = (size_t)net * a.M + row;
       float lp = 0.f;
       if (row < a.M) {
-        if (A == 12) lp = head_actions<12>(r, b3, a, row, orow, chalf);        // the A1's action dimension: every index compile-time
+        if ((od >> 1) == 12) lp = head_actions<12>(r, b3, a, row, orow, chalf);   // the A1's action dimension: every index compile-time
         else lp = head_actions<0>(r, b3, a, row, orow, chalf);
       }
       if (a.mode == B2Q_MLP_SAMPLE && a.logp) {
@@ -292,8 +286,8 @@ __global__ void __launch_bounds__(NTHR, 1) b2q_mlp_fwd_kernel(FwdArgs a) { pdl_s
   }
   if (a.da) {
     // ---- input-gradient pass (out_dim == 1): unit output gradient back to the action columns of the input, on the same tile.
-    // (a) dh2 = W3 . relu'(h2), in place over the h2 tile (layer 3's MMAs have completed: every thread waited on bar_mma above).  Row 0 of the
-    //     W3 operand image is W3 itself: 128 contiguous bytes per 64-column panel.
+    __syncthreads();   // both warpgroups' layer-3 MMAs have read the h2 tile
+    // (a) dh2 = W3 . relu'(h2), in place over the h2 tile.  Row 0 of the W3 operand image is W3 itself: 128 contiguous bytes per 64-column panel.
 #pragma unroll 4
     for (int c0 = 128 * chalf; c0 < 128 * chalf + 128; c0 += 8) {
       uint8_t* hp = smem + OFF_A + sw128_offset(trow, c0, TILE_M);
@@ -306,70 +300,45 @@ __global__ void __launch_bounds__(NTHR, 1) b2q_mlp_fwd_kernel(FwdArgs a) { pdl_s
       *reinterpret_cast<uint4*>(hp) = make_uint4(o[0], o[1], o[2], o[3]);
     }
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    // (b) dh1 pre-mask = dh2 . W2  -> TMEM cols 256..511 (B operand: the W2^T image)
-    if (tid == 0) {
-      mbar_wait(bar_w2t, 0);
-      tc_fence_after();
-      const uint32_t idesc = umma_idesc(TILE_M, HID);
+    // (b) dh1 pre-mask = dh2 . W2  -> acc (B operand: the W2^T image)
+    mbar_wait(bar_w2t, 0);
+    mma_hidden_256(sW2);
+    mma_done();
+    // (c) dh1 = . relu'(h1) (bits kept from epilogue 1, same fragment positions) -> bf16 over this warpgroup's rows of the tile
 #pragma unroll
-      for (int ks = 0; ks < 16; ks++)
-        umma_f16(tmem + 256, umma_desc(sA + (ks >> 2) * (TILE_M * 128) + (ks & 3) * 32), umma_desc(sW2 + (ks >> 2) * (HID * 128) + (ks & 3) * 32), idesc, ks > 0);
-      umma_commit(bar_mma);
-    }
-    __syncwarp();
-    mbar_wait(bar_mma, 1);
-    tc_fence_after();
-    // (c) dh1 = . relu'(h1) (bits kept from epilogue 1) -> bf16 over the tile
+    for (int j = 0; j < 32; j++) {
+      const int c = 8 * j + fc0;
 #pragma unroll
-    for (int c4 = 0; c4 < 4; c4++) {
-      const int cc = 4 * chalf + c4;
-      uint32_t r[32];
-      __syncwarp();
-      tmem_ld32(lane_addr + 256 + cc * 32, r);
-#pragma unroll
-      for (int j0 = 0; j0 < 32; j0 += 8) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) {
-          const float v0 = ((m1[c4] >> (j0 + j)) & 1u) ? __uint_as_float(r[j0 + j]) : 0.f, v1 = ((m1[c4] >> (j0 + j + 1)) & 1u) ? __uint_as_float(r[j0 + j + 1]) : 0.f;
-          __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1);
-          pk[j >> 1] = *reinterpret_cast<uint32_t*>(&h);
-        }
-        *reinterpret_cast<uint4*>(smem + OFF_A + sw128_offset(trow, cc * 32 + j0, TILE_M)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+      for (int h = 0; h < 2; h++) {
+        const int bit = 4 * (j & 7) + 2 * h;
+        const float v0 = ((m1[j >> 3] >> bit) & 1u) ? acc[4 * j + 2 * h] : 0.f, v1 = ((m1[j >> 3] >> (bit + 1)) & 1u) ? acc[4 * j + 2 * h + 1] : 0.f;
+        *reinterpret_cast<__nv_bfloat162*>(smem + OFF_A + sw128_offset(fr0 + 8 * h, c, TILE_M)) = __floats2bfloat162_rn(v0, v1);
       }
     }
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    // (d) da = dh1 . W1[:, action]  -> TMEM cols 0..15 (B operand: the W1A image, N = 16)
-    if (tid == 0) {
-      const uint32_t idesc = umma_idesc(TILE_M, 16);
+    // (d) da = dh1 . W1[:, action]  -> accd (B operand: the W1A image, N = 16)
+    float accd[8];
 #pragma unroll
-      for (int ks = 0; ks < 16; ks++)
-        umma_f16(tmem, umma_desc(sA + (ks >> 2) * (TILE_M * 128) + (ks & 3) * 32), umma_desc(sW13 + OFF_W1A_IN_W13 + (ks >> 2) * (16 * 128) + (ks & 3) * 32), idesc, ks > 0);
-      umma_commit(bar_mma);
-    }
-    __syncwarp();
-    mbar_wait(bar_mma, 0);
-    tc_fence_after();
-    if (chalf == 0) {
-      uint32_t r[32];
-      __syncwarp();
-      tmem_ld32(lane_addr, r);          // columns 16..31 are stale head outputs: not stored
-      if (row < a.M) {
-        float4* dst = reinterpret_cast<float4*>(a.da + ((size_t)net * a.M + row) * 16);
+    for (int i = 0; i < 8; i++) accd[i] = 0.f;
+    wg_fence();
 #pragma unroll
-        for (int j = 0; j < 4; j++) dst[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
+    for (int ks = 0; ks < 16; ks++)
+      Wgmma<16>::mma(accd, wg_desc(sAw + (ks >> 2) * (TILE_M * 128) + (ks & 3) * 32), wg_desc(sW13 + OFF_W1A_IN_W13 + (ks >> 2) * (16 * 128) + (ks & 3) * 32), ks > 0);
+    wg_commit();
+    wg_wait0();
+    wg_fence_acc(accd);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int gr = row0 + fr0 + 8 * h;
+      if (gr < a.M) {
+        float* dst = a.da + ((size_t)net * a.M + gr) * 16;
+#pragma unroll
+        for (int j = 0; j < 2; j++) *reinterpret_cast<float2*>(dst + 8 * j + fc0) = make_float2(accd[4 * j + 2 * h], accd[4 * j + 2 * h + 1]);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
 }
 
 // f32 nn.Linear weights -> bf16 swizzled operand images (+ f32 biases) in the per-net image

@@ -1,5 +1,5 @@
 // b2q_mlp_internal.h — library-internal extension of the MLP forward used by the SAC trainer (b2q_sac.cu): the same
-// fused tcgen05 kernel, additionally dumping the bf16 layer inputs it already holds in shared memory, in the two layouts
+// fused wgmma kernel, additionally dumping the bf16 layer inputs it already holds in shared memory, in the two layouts
 // the backward GEMMs consume ([batch x width] and [width x batch]).  Not part of the public C ABI.
 #pragma once
 #include <cuda_bf16.h>

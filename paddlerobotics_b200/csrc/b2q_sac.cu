@@ -1,9 +1,9 @@
-// b2q_sac.cu — K5/K6: SAC update on the GPU (include/b2q_sac.h): critic + actor forward (fused tcgen05 MLP kernel of
-// b2q_mlp.cu with activation dumps), backward GEMMs on tcgen05 tensor cores, fused elementwise epilogues, Adam and Polyak.
+// b2q_sac.cu — K5/K6: SAC update on the GPU (include/b2q_sac.h): critic + actor forward (fused wgmma MLP kernel of
+// b2q_mlp.cu with activation dumps), backward GEMMs on wgmma tensor cores, fused elementwise epilogues, Adam and Polyak.
 // Reference: SAC.learn / _critic_learn / _actor_learn / sync_target, ETGRL/alg/sac.py:77-118; torch.optim.Adam :55-58.
 //
 // Every backward product is phrased as C[MxN] (+)= A[MxK] . B[NxK]^T with both operands K-major bf16 (the layout the
-// tcgen05 descriptors of b2q_tc.cuh address): weight gradients contract over the batch (K = batch, split-K across CTAs,
+// wgmma descriptors of b2q_tc.cuh address): weight gradients contract over the batch (K = batch, split-K across CTAs,
 // f32 atomics), data gradients contract over the hidden width.  Activations are therefore kept in two bf16 layouts
 // ([batch x width] and [width x batch]) written by the forward kernel's epilogue, and each weight matrix has a transposed
 // bf16 copy refreshed by the optimiser kernel.
@@ -33,11 +33,11 @@ constexpr int H = 256;
 // ---------------------------------------------------------------------------------------------------------------------
 // generic tensor-core GEMM  C[M x N] (+)= A[M x K] . B[N x K]^T   (bf16 K-major operands, f32 result), N tiled by BN <= 64
 //
-// Blackwell-native feed: both operands arrive through TMA tensor maps (cp.async.bulk.tensor.2d, SWIZZLE_128B boxes of 64 K-elements:
-// exactly the K-major shared-memory image the tcgen05 descriptors address; out-of-range rows / K are zero-filled by the TMA unit), a
-// 4-stage full/empty mbarrier ring, warp-specialised roles — warp 0 = TMA producer, warp 1 = tcgen05.mma issuer, all four warps =
-// epilogue — and an epilogue that goes TMEM -> registers -> shared memory -> fully coalesced stores (or coalesced f32 reductions for
-// the split-K weight gradients).
+// Hopper feed: both operands arrive through TMA tensor maps (cp.async.bulk.tensor.2d, SWIZZLE_128B boxes of 64 K-elements: exactly
+// the K-major shared-memory image the wgmma descriptors address; out-of-range rows / K are zero-filled by the TMA unit) into a 4-stage
+// mbarrier ring that thread 0 keeps G_NSTAGE - 1 chunks ahead of the MMAs.  One warpgroup (128 threads) issues the wgmmas for the two
+// 64-row halves of the 128-row tile (accumulators in registers), then the epilogue goes registers -> shared memory -> fully coalesced
+// stores (or coalesced f32 reductions for the split-K weight gradients).
 struct GemmArgs {
   float* C; int ldc;
   int M, N, K, BN, chunks_per_split, atomic;
@@ -55,121 +55,113 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm,
                ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(bar) : "memory");
 }
 
+// WN: the MMA width (32 or 64) covering the tile's BN columns; B rows beyond BN only feed accumulator columns that are never stored
+template <int WN>
 __global__ void __launch_bounds__(128) b2q_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmArgs g) { pdl_sync();
   extern __shared__ uint8_t smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;                 // SWIZZLE_128B operand tiles want 1024-byte alignment
   uint8_t* smem = smem_raw + (sbase - smem_u32(smem_raw));
-  const uint32_t bar_full = sbase + G_NSTAGE * G_STAGE, bar_empty = bar_full + 8 * G_NSTAGE, bar_done = bar_empty + 8 * G_NSTAGE;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + G_NSTAGE * G_STAGE + 8 * (2 * G_NSTAGE + 1) + 8);
+  const uint32_t bar_full = sbase + G_NSTAGE * G_STAGE;
   const int row0 = blockIdx.x * 128, n0 = blockIdx.y * g.BN;   // output tile: 128 rows x BN columns
   const int nk_total = (g.K + 63) / 64;
   const int kc0 = blockIdx.z * g.chunks_per_split, kc1 = min(nk_total, kc0 + g.chunks_per_split), nk = kc1 - kc0;
-  const uint32_t tm_cols = g.BN <= 32 ? 32u : 64u;
+  const uint32_t bytes = G_STAGE_A + (uint32_t)g.BN * 128u;
+  auto load = [&](int kc) {   // thread 0: chunk kc of this split into its stage
+    const int st = kc % G_NSTAGE;
+    mbar_expect_tx(bar_full + 8 * st, bytes);
+    tma_load_2d(sbase + st * G_STAGE, &tmA, (kc0 + kc) * 64, row0, bar_full + 8 * st);
+    tma_load_2d(sbase + st * G_STAGE + G_STAGE_A, &tmB, (kc0 + kc) * 64, n0, bar_full + 8 * st);
+  };
   if (tid == 0) {
-    for (int i = 0; i < G_NSTAGE; i++) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 1); }
-    mbar_init(bar_done, 1);
+    for (int i = 0; i < G_NSTAGE; i++) mbar_init(bar_full + 8 * i, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    for (int kc = 0; kc < min(nk, G_NSTAGE); kc++) load(kc);
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(const_cast<const uint32_t*>(tmem_slot))), "r"(tm_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  if (nk > 0) {
-    if (warp == 0) {
-      if (lane == 0) {   // ---- TMA producer
-        const uint32_t bytes = G_STAGE_A + (uint32_t)g.BN * 128u;
-        for (int kc = 0; kc < nk; kc++) {
-          const int st = kc % G_NSTAGE;
-          if (kc >= G_NSTAGE) mbar_wait(bar_empty + 8 * st, (uint32_t)((kc / G_NSTAGE - 1) & 1));
-          mbar_expect_tx(bar_full + 8 * st, bytes);
-          tma_load_2d(sbase + st * G_STAGE, &tmA, (kc0 + kc) * 64, row0, bar_full + 8 * st);
-          tma_load_2d(sbase + st * G_STAGE + G_STAGE_A, &tmB, (kc0 + kc) * 64, n0, bar_full + 8 * st);
-        }
-      }
-      __syncwarp();
-    } else if (warp == 1) {
-      if (lane == 0) {   // ---- MMA issuer
-        const uint32_t idesc = umma_idesc(128, g.BN);
-        for (int kc = 0; kc < nk; kc++) {
-          const int st = kc % G_NSTAGE;
-          mbar_wait(bar_full + 8 * st, (uint32_t)((kc / G_NSTAGE) & 1));
-          tc_fence_after();
-          const uint32_t sa = sbase + st * G_STAGE, sb = sa + G_STAGE_A;
+  if (nk <= 0) return;
+  // accumulator fragments of the two 64-row halves (b2q_tc.cuh: d[4 j + 2 h + e] = row 16 warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e)
+  float acc[2][WN / 2];
 #pragma unroll
-          for (int ks = 0; ks < 4; ks++) umma_f16(tmem, umma_desc(sa + ks * 32), umma_desc(sb + ks * 32), idesc, (kc > 0 || ks > 0) ? 1u : 0u);
-          umma_commit(bar_empty + 8 * st);          // frees the stage when these MMAs have read it
-        }
-        umma_commit(bar_done);
-      }
-      __syncwarp();
+  for (int m = 0; m < 2; m++)
+#pragma unroll
+    for (int i = 0; i < WN / 2; i++) acc[m][i] = 0.f;
+  for (int kc = 0; kc < nk; kc++) {
+    const int st = kc % G_NSTAGE;
+    mbar_wait(bar_full + 8 * st, (uint32_t)((kc / G_NSTAGE) & 1));
+    const uint32_t sa = sbase + st * G_STAGE, sb = sa + G_STAGE_A;
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ks++)
+#pragma unroll
+      for (int m = 0; m < 2; m++) Wgmma<WN>::mma(acc[m], wg_desc(sa + m * 64 * 128 + ks * 32), wg_desc(sb + ks * 32), (kc > 0 || ks > 0) ? 1u : 0u);
+    wg_commit();
+    wg_wait0();
+    wg_fence_acc(acc[0]); wg_fence_acc(acc[1]);
+    if (kc + G_NSTAGE < nk) {
+      __syncthreads();                                   // every warp's MMAs have read the stage before it is refilled
+      if (tid == 0) load(kc + G_NSTAGE);
     }
-    // ---- epilogue (all four warps): TMEM lane = tile row; stage the tile in shared memory, then coalesced stores / reductions
-    mbar_wait(bar_done, 0);
-    tc_fence_after();
-    if (g.mask_h) {
-      constexpr int LDR = 72, LDT = 136;                                  // bf16 elements per staged row: 16-byte aligned, conflict-free for the accesses below
-      bf16* t_rm = reinterpret_cast<bf16*>(smem);                          // [128][LDR]  rows x this CTA's 64 columns
-      bf16* t_t = reinterpret_cast<bf16*>(smem + 128 * LDR * 2);           // [64][LDT]   columns x 128 rows
-      const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
-      const bf16* hrow = g.mask_h + (size_t)(row0 + tid) * g.N + n0;
+  }
+  __syncthreads();                                       // the operand ring is drained: the epilogue reuses it as its staging tile
+  const int fr = 16 * warp + (lane >> 2), fc = 2 * (lane & 3);
+  if (g.mask_h) {
+    constexpr int LDR = 72, LDT = 136;                                  // bf16 elements per staged row: 16-byte aligned
+    bf16* t_rm = reinterpret_cast<bf16*>(smem);                          // [128][LDR]  rows x this CTA's 64 columns
+    bf16* t_t = reinterpret_cast<bf16*>(smem + 128 * LDR * 2);           // [64][LDT]   columns x 128 rows
 #pragma unroll
-      for (int cc = 0; cc < 2; cc++) {
-        uint32_t r[32];
-        uint4 hv[4];
+    for (int m = 0; m < 2; m++)
 #pragma unroll
-        for (int q = 0; q < 4; q++) hv[q] = *reinterpret_cast<const uint4*>(hrow + cc * 32 + q * 8);
-        __syncwarp();
-        tmem_ld32(lane_addr + cc * 32, r);
+      for (int h = 0; h < 2; h++) {
+        const int r_ = 64 * m + fr + 8 * h;
+        const bf16* hrow = g.mask_h + (size_t)(row0 + r_) * g.N + n0;
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
-          const bf16* hb = reinterpret_cast<const bf16*>(&hv[q]);
-          __align__(16) bf16 o[8];
-#pragma unroll
-          for (int j = 0; j < 8; j++) {
-            o[j] = __float2bfloat16(__bfloat162float(hb[j]) > 0.f ? __uint_as_float(r[q * 8 + j]) : 0.f);
-            t_t[(cc * 32 + q * 8 + j) * LDT + tid] = o[j];
-          }
-          *reinterpret_cast<uint4*>(t_rm + tid * LDR + cc * 32 + q * 8) = *reinterpret_cast<const uint4*>(o);
+        for (int j = 0; j < WN / 8; j++) {
+          const int c_ = 8 * j + fc;
+          const __nv_bfloat162 hv = *reinterpret_cast<const __nv_bfloat162*>(hrow + c_);
+          const bf16 o0 = __float2bfloat16(__bfloat162float(hv.x) > 0.f ? acc[m][4 * j + 2 * h] : 0.f);
+          const bf16 o1 = __float2bfloat16(__bfloat162float(hv.y) > 0.f ? acc[m][4 * j + 2 * h + 1] : 0.f);
+          __nv_bfloat162 o; o.x = o0; o.y = o1;
+          *reinterpret_cast<__nv_bfloat162*>(t_rm + r_ * LDR + c_) = o;
+          t_t[c_ * LDT + r_] = o0; t_t[(c_ + 1) * LDT + r_] = o1;
         }
       }
-      __syncthreads();
-      if (g.dh_rm)
-        for (int i = tid; i < 128 * 8; i += 128) { const int r_ = i >> 3, sg = i & 7;
-          *reinterpret_cast<uint4*>(g.dh_rm + (size_t)(row0 + r_) * g.N + n0 + sg * 8) = *reinterpret_cast<const uint4*>(t_rm + r_ * LDR + sg * 8); }
-      if (g.dh_t)
-        for (int i = tid; i < 64 * 16; i += 128) { const int c_ = i >> 4, sg = i & 15;
-          *reinterpret_cast<uint4*>(g.dh_t + (size_t)(n0 + c_) * g.M + row0 + sg * 8) = *reinterpret_cast<const uint4*>(t_t + c_ * LDT + sg * 8); }
-      if (g.db) {                                                          // column sums of the rounded values (what the weight-gradient GEMMs see)
-        const int c_ = tid >> 1, hf = tid & 1;
-        float sum = 0.f;
+    __syncthreads();
+    if (g.dh_rm)
+      for (int i = tid; i < 128 * 8; i += 128) { const int r_ = i >> 3, sg = i & 7;
+        *reinterpret_cast<uint4*>(g.dh_rm + (size_t)(row0 + r_) * g.N + n0 + sg * 8) = *reinterpret_cast<const uint4*>(t_rm + r_ * LDR + sg * 8); }
+    if (g.dh_t)
+      for (int i = tid; i < 64 * 16; i += 128) { const int c_ = i >> 4, sg = i & 15;
+        *reinterpret_cast<uint4*>(g.dh_t + (size_t)(n0 + c_) * g.M + row0 + sg * 8) = *reinterpret_cast<const uint4*>(t_t + c_ * LDT + sg * 8); }
+    if (g.db) {                                                          // column sums of the rounded values (what the weight-gradient GEMMs see)
+      const int c_ = tid >> 1, hf = tid & 1;
+      float sum = 0.f;
 #pragma unroll
-        for (int k = 0; k < 8; k++) {
-          const uint4 v = *reinterpret_cast<const uint4*>(t_t + c_ * LDT + hf * 64 + k * 8);
-          const bf16* vb = reinterpret_cast<const bf16*>(&v);
+      for (int k = 0; k < 8; k++) {
+        const uint4 v = *reinterpret_cast<const uint4*>(t_t + c_ * LDT + hf * 64 + k * 8);
+        const bf16* vb = reinterpret_cast<const bf16*>(&v);
 #pragma unroll
-          for (int j = 0; j < 8; j++) sum += __bfloat162float(vb[j]);
-        }
-        sum += __shfl_xor_sync(0xffffffffu, sum, 1);
-        if (hf == 0) atomicAdd(g.db + n0 + c_, sum);
+        for (int j = 0; j < 8; j++) sum += __bfloat162float(vb[j]);
       }
-    } else {
-    float* stile = reinterpret_cast<float*>(smem);                      // [128][BN + 1] floats: the operand ring is drained by now
+      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+      if (hf == 0) atomicAdd(g.db + n0 + c_, sum);
+    }
+  } else {
+    float* stile = reinterpret_cast<float*>(smem);                      // [128][BN + 1] floats
     const int ldt = g.BN + 1;
-    const uint32_t lane_addr = tmem + ((uint32_t)(warp * 32) << 16);
-    for (int cc = 0; cc < (g.BN + 31) / 32; cc++) {
-      uint32_t r[32];
-      __syncwarp();
-      tmem_ld32(lane_addr + cc * 32, r);
 #pragma unroll
-      for (int j = 0; j < 32; j++) if (cc * 32 + j < g.BN) stile[tid * ldt + cc * 32 + j] = __uint_as_float(r[j]);
-    }
+    for (int m = 0; m < 2; m++)
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int j = 0; j < WN / 8; j++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int c_ = 8 * j + fc + e;
+            if (c_ < g.BN) stile[(64 * m + fr + 8 * h) * ldt + c_] = acc[m][4 * j + 2 * h + e];
+          }
     __syncthreads();
     const int ncol = min(g.BN, g.N - n0), nrow = min(128, g.M - row0);
     for (int i = tid; i < nrow * ncol; i += 128) {
@@ -178,11 +170,7 @@ __global__ void __launch_bounds__(128) b2q_gemm_kernel(const __grid_constant__ C
       const float v = stile[r_ * ldt + c_];
       if (g.atomic) atomicAdd(c, v); else *c = v;
     }
-    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tm_cols) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -515,7 +503,8 @@ int gemm(B2QSac* s, cudaStream_t st, const bf16* A, int lda, const bf16* Bm, int
   if (!ta || !tb) { s->err = "cuTensorMapEncodeTiled failed"; return -2; }
   // split-K products accumulate with f32 atomics: C must be zero on entry (every caller targets the gradient bucket, cleared once per learn)
   dim3 grid((M + 127) / 128, ntiles, splits);
-  pdl_launch(b2q_gemm_kernel, dim3(grid), dim3(128), G_SMEM, st, *ta, *tb, g);
+  if (g.BN <= 32) pdl_launch(b2q_gemm_kernel<32>, dim3(grid), dim3(128), G_SMEM, st, *ta, *tb, g);
+  else pdl_launch(b2q_gemm_kernel<64>, dim3(grid), dim3(128), G_SMEM, st, *ta, *tb, g);
   s->launches++;
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
@@ -635,7 +624,8 @@ int b2q_sac_create(int device, int obs_dim, int act_dim, int batch, float gamma,
   ok = ok && b2q_mlp_create(device, obs_dim, 2 * act_dim, 1, &s->mlp_actor) == 0 && b2q_mlp_create(device, obs_dim + act_dim, 1, 2, &s->mlp_critic) == 0 &&
        b2q_mlp_create(device, obs_dim + act_dim, 1, 2, &s->mlp_target) == 0 &&
        b2q_mlp_set_action_slice(s->mlp_critic, obs_dim, act_dim) == 0;
-  ok = ok && cudaFuncSetAttribute(b2q_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM) == cudaSuccess;
+  ok = ok && cudaFuncSetAttribute(b2q_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM) == cudaSuccess &&
+       cudaFuncSetAttribute(b2q_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM) == cudaSuccess;
   if (!ok) { b2q_sac_destroy(s); return -3; }
   *out = s;
   return 0;

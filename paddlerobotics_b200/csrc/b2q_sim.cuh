@@ -675,8 +675,8 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
   }
   } else {
   // float64 validation build: the fully redundant build (every lane gathers all rows with 4-lane broadcasts and forms the whole matrix);
-  // measured on B200 the shared-memory exchange above is 4.6 % faster in f32 but 1.8x slower in f64 (twice the shared-memory traffic
-  // next to a saturated FP64 pipe), so each precision keeps the variant that is faster for it
+  // the shared-memory exchange above is the f32 choice; in f64 it moves twice the shared-memory traffic next to a saturated FP64 pipe,
+  // so the f64 build keeps this shuffle-only variant
   // --- gather every foot's rows on every lane (4-lane broadcasts), then the whole 12x12 contact problem is solved
   //     REDUNDANTLY in registers by all four lanes: the Gauss-Seidel sweep below has no shuffle on its dependent chain.
   //     Row index r = 3*foot + e (e: 0 normal, 1,2 friction).
@@ -697,10 +697,9 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     lam[3 * f + 1] = T(0); lam[3 * f + 2] = T(0);
   }
   // Delassus matrix W = J M^-1 J^T (symmetric): W_ij = Y_i . Y_j (+ the leg-local 3x3 block on the diagonal blocks), built
-  // directly in the layout the sweep consumes — PAIRS of adjacent rows — with the packed FP32 FMA of sm_100 (FFMA2, scalar
-  // broadcast operand): WR[r][p] = (W[2p][r], W[2p+1][r]).  Only the pairs at or below the diagonal are computed (42 x 6
-  // packed FMAs instead of 78 x 6 scalar ones); the rest are re-paired from them by symmetry.  The substep body is
-  // instruction-FETCH bound (57 KB of straight-line code per substep, DESIGN.md §5), so instruction count is what matters.
+  // directly in the layout the sweep consumes — PAIRS of adjacent rows, scalar broadcast operand: WR[r][p] = (W[2p][r], W[2p+1][r]).
+  // Only the pairs at or below the diagonal are computed (42 x 6 pair FMAs instead of 78 x 6 for the full matrix); the rest are
+  // re-paired from them by symmetry.  The substep body is straight-line code, so instruction count is what matters.
   P2<T> WR[12][6];
   {
     P2<T> YP[6][6];
@@ -765,8 +764,6 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
   }
   // --- projected Gauss-Seidel, Bullet row order: normals of feet 0..3, then (t1,t2) of feet 0..3.
   //     Row update = clamp -> delta -> 11 independent scalar FFMAs (W'_rr = 0: the row's own candidate is unchanged).
-  //     Plain FFMAs on purpose: the packed FFMA2 issues at half rate for a single warp and lengthens the serial chain
-  //     clamp(r) -> g(r+1) -> clamp(r+1) (microbenchmark scripts/ubench/ffma2.cu: 17.0 vs 22.8 cycles per row; DESIGN.md §5).
   for (int it = 0; it < cf.iters; it++) {
 #pragma unroll
     for (int f = 0; f < 4; f++) {

@@ -1,7 +1,7 @@
 """ETG-RL training loop on the GPU engine — the batched counterpart of ETGRL/train.py:252-449 (same phases, same flag names
 where they exist): SAC episodes with one learner step per control step (train.py:163-169) over N parallel envs, and every
 `ES_EVERY_STEPS` env steps an ES phase of `ES_TRAIN_STEPS` generations over the ETG control points (train.py:392-437).
-Everything per-step stays on the device: obs -> fused MLP (tcgen05) -> step kernel -> device replay -> SAC learn (CUDA graph).
+Everything per-step stays on the device: obs -> fused MLP (wgmma) -> step kernel -> device replay -> SAC learn (CUDA graph).
 
     python -m paddlerobotics_b200.train --num_envs 4096 --max_steps 2000000 --ES 1
 """

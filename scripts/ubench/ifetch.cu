@@ -32,7 +32,7 @@ void run(int grid) {
   cudaFree(out); cudaFree(cyc); delete[] h;
 }
 int main() {
-  for (int grid : {148, 592, 1184, 2368}) {
+  for (int grid : {132, 528, 1056, 2112}) {
     run<256>(grid); run<1024>(grid); run<1792>(grid); run<2304>(grid); run<3584>(grid); run<7168>(grid);
   }
   return 0;

@@ -1,6 +1,6 @@
 """The DEVICE code of the step kernel (paddlerobotics_b200/csrc/b2q_sim.cuh), compiled for the CPU with the warp
 shuffles replaced by a 4-thread lock-step exchange (tests/emu/), against the float64 oracle.  This is the CPU-side
-check of the kernel logic; the `-m gpu` tests repeat it through the real C ABI on the B200."""
+check of the kernel logic; the `-m gpu` tests repeat it through the real C ABI on the H100."""
 import sys
 import os
 

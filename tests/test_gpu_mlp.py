@@ -1,4 +1,4 @@
-"""K3: fused tcgen05 MLP forward vs a plain PyTorch fp32 reference of the same op, and vs the known answers of the
+"""K3: fused wgmma MLP forward vs a plain PyTorch fp32 reference of the same op, and vs the known answers of the
 reference's shipped checkpoint (tests/golden/StairStair3_BC1_itr_500383.pt; vectors made by the unmodified
 model/mujoco_model.py).  Arithmetic is bf16 x bf16 -> f32 (BASELINE: bf16 tensor-core GEMM), so the tolerance is the
 bf16 one: |err| <= 2e-2 + 3e-2*max(1,|ref|) on pre-activations of the trained checkpoint (measured 4e-2 at |ref|~1.5),

@@ -1,5 +1,5 @@
 """K5/K6: SAC.learn on the device vs a plain PyTorch fp32 restatement of ETGRL/alg/sac.py:77-118 (same minibatch, same
-N(0,1) draws for both rsample() calls).  Forward/backward GEMMs run in bf16 on tcgen05 with f32 accumulation, so the
+N(0,1) draws for both rsample() calls).  Forward/backward GEMMs run in bf16 on wgmma tensor cores with f32 accumulation, so the
 tolerance is the bf16 one: losses within 2 %, gradient buckets within 5 % relative L2 error and cosine >= 0.995."""
 import numpy as np
 import pytest
