@@ -17,7 +17,7 @@ namespace {
 
 struct WarpComm {
   int k;
-  unsigned char* scr;   // this robot's shared-memory scratch (FEAT variant only; null otherwise)
+  unsigned char* scr;   // this robot's shared-memory scratch, scratch_floats(FEAT) elements (null in the reset kernel)
   __device__ __forceinline__ int leg() const { return k; }
   template <typename T> __device__ __forceinline__ T* scratch() const { return reinterpret_cast<T*>(scr); }
   __device__ __forceinline__ void sync() const { __syncwarp(); }
@@ -30,8 +30,6 @@ struct WarpComm {
   }
   template <typename T>
   __device__ __forceinline__ T bcast(T v, int f) const { return __shfl_sync(0xffffffffu, v, f, 4); }
-  template <typename T> __device__ __forceinline__ T xor1(T v) const { return __shfl_xor_sync(0xffffffffu, v, 1); }   // partner lanes of the
-  template <typename T> __device__ __forceinline__ T xor2(T v) const { return __shfl_xor_sync(0xffffffffu, v, 2); }   // 4-lane butterfly
 };
 
 template <typename T>
@@ -95,7 +93,7 @@ __global__ void __launch_bounds__(128) b2q_step_kernel(Cfg<T> cf, const Model<T>
   const int srow = env0 + (int)(threadIdx.x >> 2);
   if (!valid) env = B.N - 1;
   T* istage0 = stage + (size_t)per_cta * OBS_DIM;
-  WarpComm cm{(int)(threadIdx.x & 3), reinterpret_cast<unsigned char*>(istage0 + (size_t)per_cta * INFO_DIM + (size_t)(threadIdx.x >> 2) * (FEAT ? SCRATCH_FLOATS : (sizeof(T) == 4 ? SCRATCH_FAST : 0)))};
+  WarpComm cm{(int)(threadIdx.x & 3), reinterpret_cast<unsigned char*>(istage0 + (size_t)per_cta * INFO_DIM + (size_t)(threadIdx.x >> 2) * scratch_floats(FEAT))};
   // the info rows (56 floats per env, produced in 3-float pieces) are staged the same way: one coalesced block per CTA, so that `info`
   // too may be pinned HOST memory (train.py:150-157 reads info every step)
   T* istage = istage0;
@@ -116,7 +114,7 @@ __global__ void __launch_bounds__(128) b2q_settle_kernel(Cfg<T> cf, const Model<
   if (!valid) env = B.N - 1;
   if (mask && !mask[env]) valid = false;
   T* scr0 = reinterpret_cast<T*>(smem + ((sizeof(Model<T>) + 31) & ~size_t(31))) + (size_t)(blockDim.x >> 2) * (OBS_DIM + INFO_DIM);
-  WarpComm cm{(int)(threadIdx.x & 3), reinterpret_cast<unsigned char*>(scr0 + (size_t)(threadIdx.x >> 2) * (FEAT ? SCRATCH_FLOATS : (sizeof(T) == 4 ? SCRATCH_FAST : 0)))};
+  WarpComm cm{(int)(threadIdx.x & 3), reinterpret_cast<unsigned char*>(scr0 + (size_t)(threadIdx.x >> 2) * scratch_floats(FEAT))};
   settle_lane<T, FEAT>(cm, cf, md, B, env, valid);
 }
 
@@ -280,8 +278,8 @@ struct EnvT : EnvBase {
     CK(cudaDeviceSynchronize());
     return B2Q_OK;
   }
-  size_t smem_bytes() const {   // model | obs stage | info stage | (FEAT) per-robot solver scratch
-    return ((sizeof(Model<T>) + 31) & ~size_t(31)) + (size_t)(tpb / 4) * (OBS_DIM + INFO_DIM + (feat ? SCRATCH_FLOATS : (sizeof(T) == 4 ? SCRATCH_FAST : 0))) * sizeof(T);   // the f64 build exchanges through shuffles: no scratch, so its spill traffic keeps the L1
+  size_t smem_bytes() const {   // model | obs stage | info stage | per-robot solver scratch
+    return ((sizeof(Model<T>) + 31) & ~size_t(31)) + (size_t)(tpb / 4) * (OBS_DIM + INFO_DIM + scratch_floats(feat)) * sizeof(T);
   }
 
   int set_dynamics(const uint8_t* mask, const void* dyn, cudaStream_t s) override {

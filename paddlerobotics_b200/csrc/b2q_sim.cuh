@@ -200,6 +200,9 @@ B2Q_HD void etg_act_leg(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, co
 constexpr int RPL = 9, NRW = 4 * RPL;
 constexpr int SCRATCH_FLOATS = NRW * 6 + 4 * 45 + NRW * 4 + NRW * NRW;
 constexpr int SCRATCH_FAST = 272;   // the default body's exchange area: Y^T [6][12] | vectors [4][12] | active [4] (+pad) | W' [12][12]
+// elements of T in one robot's shared scratch.  Its size and the offsets of its areas are multiples of 4 elements, so the P4<T> loads and
+// stores of the exchange stay aligned in both precisions whenever the first robot's scratch is.
+B2Q_HD constexpr int scratch_floats(int feat) { return feat ? SCRATCH_FLOATS : SCRATCH_FAST; }
 #define JLIM_GAP T(0.06)
 template <typename T, class Comm>
 B2Q_HD void solve_rows36(const Comm& cm, const Cfg<T>& cf, T mu, const T (*Y)[6] /*[9] rows of this leg*/, const T* u /*[9]*/, const T* blk45 /*leg-local 9x9 block, packed lower*/,
@@ -350,22 +353,17 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     D[2][2] = (M11 * M22 - M21 * M21) * id;
   }
   T bj[3] = {tau[0] - hj[0], tau[1] - hj[1], tau[2] - hj[2]};
-  // F_k D_k (6x3) and the leg's Schur contribution C_k - (F D) F^T as PAIRS of adjacent components with the packed FP32 ops
-  // (the body is instruction-fetch bound, DESIGN.md §5): FP[i][p] = (F_i[2p], F_i[2p+1]), FDP[j][p] likewise.
-  P2<T> FP[3][3], FDP[3][3];
+  // F_k (as arrays: Fa[i][c] = component c of column i) and F_k D_k (6x3): FD[j][c] = sum_i F_i[c] D[i][j]
+  T Fa[3][6], FD[3][6];
 #pragma unroll
-  for (int i = 0; i < 3; i++) { FP[i][0] = p2mk(Fc[i].a.x, Fc[i].a.y); FP[i][1] = p2mk(Fc[i].a.z, Fc[i].l.x); FP[i][2] = p2mk(Fc[i].l.y, Fc[i].l.z); }
+  for (int i = 0; i < 3; i++) v6_to_arr(Fc[i], Fa[i]);
 #pragma unroll
   for (int j = 0; j < 3; j++) {
 #pragma unroll
-    for (int p = 0; p < 3; p++) FDP[j][p] = p2fma(FP[2][p], p2s(D[2][j]), p2fma(FP[1][p], p2s(D[1][j]), p2mul(FP[0][p], p2s(D[0][j]))));
+    for (int c = 0; c < 6; c++) FD[j][c] = m_fma(Fa[2][c], D[2][j], m_fma(Fa[1][c], D[1][j], Fa[0][c] * D[0][j]));
   }
-#define FDA(k, i) (((i) & 1) ? FDP[k][(i) >> 1].y : FDP[k][(i) >> 1].x)
-  V6<T> FD[3];
-#pragma unroll
-  for (int j = 0; j < 3; j++) { FD[j].a = mk<T>(FDA(j, 0), FDA(j, 1), FDA(j, 2)); FD[j].l = mk<T>(FDA(j, 3), FDA(j, 4), FDA(j, 5)); }
 
-  // --- leg contribution to the base Schur complement and rhs; reduce over the 4 legs (4-lane butterflies on pairs)
+  // --- leg contribution C_k - (F D) F^T to the base Schur complement and rhs; reduce over the 4 legs (4-lane butterflies)
   T S[21], r6[6];
   {
     // composite C1 as 6x6: [[I1c, hx],[hx^T, m 1]], hx = skew(h1c); lower-left block = hx^T = [[0,hz,-hy],[-hz,0,hx],[hy,-hx,0]]
@@ -379,25 +377,20 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
 #pragma unroll
     for (int i = 0; i < 6; i++) {
 #pragma unroll
-      for (int p = 0; 2 * p <= i; p++) {   // columns (2p, 2p+1) of row i; for even i the last pair's second half is the mirror entry (unused)
-        P2<T> v = p2mk(Cf[i][2 * p], Cf[i][2 * p + 1]);
+      for (int j = 0; j <= i; j++) {
+        T v = Cf[i][j];
 #pragma unroll
-        for (int k = 0; k < 3; k++) v = p2fma(FP[k][p], p2s(-FDA(k, i)), v);
-        v = p2add(v, p2mk(cm.xor1(v.x), cm.xor1(v.y)));
-        v = p2add(v, p2mk(cm.xor2(v.x), cm.xor2(v.y)));
-        S[tri(i, 2 * p)] = v.x;
-        if (2 * p + 1 <= i) S[tri(i, 2 * p + 1)] = v.y;
+        for (int k = 0; k < 3; k++) v = m_fma(Fa[k][j], -FD[k][i], v);
+        S[tri(i, j)] = cm.sum4(v);
       }
     }
     const T NOa[6] = {NO.x, NO.y, NO.z, F1.x, F1.y, F1.z};
 #pragma unroll
-    for (int p = 0; p < 3; p++) {
-      P2<T> v = p2mk(-NOa[2 * p], -NOa[2 * p + 1]);
+    for (int i = 0; i < 6; i++) {
+      T v = -NOa[i];
 #pragma unroll
-      for (int k = 0; k < 3; k++) v = p2fma(FDP[k][p], p2s(-bj[k]), v);
-      v = p2add(v, p2mk(cm.xor1(v.x), cm.xor1(v.y)));
-      v = p2add(v, p2mk(cm.xor2(v.x), cm.xor2(v.y)));
-      r6[2 * p] = v.x; r6[2 * p + 1] = v.y;
+      for (int k = 0; k < 3; k++) v = m_fma(FD[k][i], -bj[k], v);
+      r6[i] = cm.sum4(v);
     }
   }
   {
@@ -451,11 +444,11 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
       u[e] = dot(Jb.a, wBs) + dot(Jb.l, vBs) + Jk[e][0] * qds[0] + Jk[e][1] * qds[1] + Jk[e][2] * qds[2];
       const T Jba[6] = {Jb.a.x, Jb.a.y, Jb.a.z, Jb.l.x, Jb.l.y, Jb.l.z};
 #pragma unroll
-      for (int p = 0; p < 3; p++) {
-        P2<T> g = p2mk(Jba[2 * p], Jba[2 * p + 1]);
+      for (int c = 0; c < 6; c++) {
+        T g = Jba[c];
 #pragma unroll
-        for (int j = 0; j < 3; j++) g = p2fma(FDP[j][p], p2s(-Jk[e][j]), g);
-        Y[e][2 * p] = g.x; Y[e][2 * p + 1] = g.y;
+        for (int j = 0; j < 3; j++) g = m_fma(FD[j][c], -Jk[e][j], g);
+        Y[e][c] = g;
       }
       fwd6(S, Li, Y[e]);
     }
@@ -468,7 +461,6 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
       for (int e2 = 0; e2 < 3; e2++) Wl[e2][e] = Jk[e2][0] * dj[0] + Jk[e2][1] * dj[1] + Jk[e2][2] * dj[2];
     }
   }
-#undef FDA
   T lk[3] = {T(0), T(0), T(0)};   // this lane's own toe impulses
   // extra rows of this leg in the FEAT variant: knee contact (n, t1, t2) and the three joint-limit rows: impulses, base-space Y rows, joint-space Jacobians
   T lkx[6] = {T(0), T(0), T(0), T(0), T(0), T(0)}, Yx[6][6], Jx[6][3];
@@ -520,7 +512,7 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
           V6<T> Jb; Jb.a = cross(xk, ek[e]); Jb.l = ek[e];
           u9[3 + e] = dot(Jb.a, wBs) + dot(Jb.l, vBs) + jr[0] * qds[0] + jr[1] * qds[1] + jr[2] * qds[2];
 #pragma unroll
-          for (int i = 0; i < 6; i++) Yx[e][i] = get6(Jb, i) - (get6(FD[0], i) * jr[0] + get6(FD[1], i) * jr[1] + get6(FD[2], i) * jr[2]);
+          for (int i = 0; i < 6; i++) Yx[e][i] = get6(Jb, i) - (FD[0][i] * jr[0] + FD[1][i] * jr[1] + FD[2][i] * jr[2]);
           fwd6(S, Li, Yx[e]);
           Jx[e][0] = jr[0]; Jx[e][1] = jr[1]; Jx[e][2] = jr[2];
           targ9[3 + e] = T(0); warm9[3 + e] = T(0); act9[3 + e] = kact;
@@ -534,7 +526,7 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
         T glo = s.q[j] - md.qlo[j], ghi = md.qhi[j] - s.q[j], gap = glo, sj = T(1);
         if (ghi < glo) { gap = ghi; sj = T(-1); }
 #pragma unroll
-        for (int i = 0; i < 6; i++) Yx[3 + j][i] = -sj * get6(FD[j], i);
+        for (int i = 0; i < 6; i++) Yx[3 + j][i] = -sj * FD[j][i];
         fwd6(S, Li, Yx[3 + j]);
         Jx[3 + j][0] = j == 0 ? sj : T(0); Jx[3 + j][1] = j == 1 ? sj : T(0); Jx[3 + j][2] = j == 2 ? sj : T(0);
         u9[6 + j] = sj * qds[j];
@@ -567,18 +559,16 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     }
   }
   if (!general) {
-  P2<T> g2[6], Wc[12][6];
-  T lam[12];
-  if constexpr (sizeof(T) == 4) {
+  T g[12], Wc[12][12], lam[12];
   // --- the 12x12 contact problem of the robot, built ONCE by its four lanes together and then solved REDUNDANTLY in registers by all
   //     of them (the Gauss-Seidel sweep below has no shuffle on its dependent chain).  Row index r = 3*foot + e (e: 0 normal, 1,2 friction).
   //     Delassus matrix W = J M^-1 J^T: W_ij = Y_i . Y_j (+ the leg-local 3x3 block on the diagonal blocks).  The sweep consumes
-  //     W'_ir = W_ir / W_ii (zero diagonal) as PAIRS of adjacent target rows: Wc[r][p] = (W'[2p][r], W'[2p+1][r]).
-  //     Each lane publishes its foot's three Y rows (transposed, so that the others read them as target pairs), 1/W_ii, the unconstrained
-  //     velocities, target and warm start in the robot's shared scratch; after one exchange it builds the three COLUMNS of W' that belong
-  //     to its own source rows (108 packed FMAs instead of the 252 of a fully redundant build), publishes them, and after the second
-  //     exchange every lane loads the whole matrix with 128-bit loads.  (The substep body is instruction-FETCH bound — DESIGN.md §5 —
-  //     so instruction count is what matters; the two exchanges replace 120 shuffles.)
+  //     W'_ir = W_ir / W_ii (zero diagonal) by source row: Wc[r][i] = W'_ir.
+  //     Each lane publishes its foot's three Y rows (transposed, so that the others read them with four-wide vector loads), 1/W_ii, the
+  //     unconstrained velocities, target and warm start in the robot's shared scratch; after one exchange it builds the three COLUMNS of W'
+  //     that belong to its own source rows (216 multiply-adds, a quarter of the whole matrix's), publishes them, and after the second
+  //     exchange every lane loads the whole matrix with four-wide vector loads.  (The substep body is instruction-FETCH bound — DESIGN.md §5
+  //     — so instruction count is what matters; the two exchanges replace 120 shuffles.)  Both precisions run this build.
   {
     T* sh = cm.template scratch<T>();
     T* YT = sh;            // [6][12]  YT[c][i] = component c of row i's Y
@@ -602,30 +592,30 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     afs[k] = act ? T(1) : T(0);
     cm.sync();
     {
-      P2<T> YP[6][6], invp[6];   // YP[p][c] = (Y_2p[c], Y_2p+1[c])
+      T Ya[12][6], inv[12];   // Ya[i][c] = component c of row i's Y, inv[i] = 1/W_ii
 #pragma unroll
       for (int c = 0; c < 6; c++) {
 #pragma unroll
         for (int q = 0; q < 3; q++) {
           const P4<T> v = *reinterpret_cast<const P4<T>*>(YT + c * 12 + 4 * q);
-          YP[2 * q][c] = p2mk(v.x, v.y); YP[2 * q + 1][c] = p2mk(v.z, v.w);
+          Ya[4 * q][c] = v.x; Ya[4 * q + 1][c] = v.y; Ya[4 * q + 2][c] = v.z; Ya[4 * q + 3][c] = v.w;
         }
       }
 #pragma unroll
-      for (int q = 0; q < 3; q++) { const P4<T> v = *reinterpret_cast<const P4<T>*>(vecs + 4 * q); invp[2 * q] = p2mk(v.x, v.y); invp[2 * q + 1] = p2mk(v.z, v.w); }
+      for (int q = 0; q < 3; q++) { const P4<T> v = *reinterpret_cast<const P4<T>*>(vecs + 4 * q); inv[4 * q] = v.x; inv[4 * q + 1] = v.y; inv[4 * q + 2] = v.z; inv[4 * q + 3] = v.w; }
 #pragma unroll
       for (int e = 0; e < 3; e++) {          // column r = 3k + e of W': all twelve targets
         const int r = 3 * k + e;
-        P2<T> col[6];
+        T col[12];
 #pragma unroll
-        for (int p = 0; p < 6; p++) {
-          P2<T> acc = p2mul(YP[p][0], p2s(Y[e][0]));
+        for (int i = 0; i < 12; i++) {
+          T acc = Ya[i][0] * Y[e][0];
 #pragma unroll
-          for (int c = 1; c < 6; c++) acc = p2fma(YP[p][c], p2s(Y[e][c]), acc);
-          col[p] = p2mul(acc, invp[p]);
+          for (int c = 1; c < 6; c++) acc = m_fma(Ya[i][c], Y[e][c], acc);
+          col[i] = acc * inv[i];
         }
 #pragma unroll
-        for (int q = 0; q < 3; q++) { P4<T> v; v.x = col[2 * q].x; v.y = col[2 * q].y; v.z = col[2 * q + 1].x; v.w = col[2 * q + 1].y; *reinterpret_cast<P4<T>*>(Wp + r * 12 + 4 * q) = v; }
+        for (int q = 0; q < 3; q++) { P4<T> v; v.x = col[4 * q]; v.y = col[4 * q + 1]; v.z = col[4 * q + 2]; v.w = col[4 * q + 3]; *reinterpret_cast<P4<T>*>(Wp + r * 12 + 4 * q) = v; }
         // the three targets of the lane's own foot also carry the leg-local block (and the zero diagonal): overwrite them
 #pragma unroll
         for (int e2 = 0; e2 < 3; e2++) {
@@ -640,7 +630,7 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
 #pragma unroll
     for (int r = 0; r < 12; r++) {
 #pragma unroll
-      for (int q = 0; q < 3; q++) { const P4<T> v = *reinterpret_cast<const P4<T>*>(Wp + r * 12 + 4 * q); Wc[r][2 * q] = p2mk(v.x, v.y); Wc[r][2 * q + 1] = p2mk(v.z, v.w); }
+      for (int q = 0; q < 3; q++) { const P4<T> v = *reinterpret_cast<const P4<T>*>(Wp + r * 12 + 4 * q); Wc[r][4 * q] = v.x; Wc[r][4 * q + 1] = v.y; Wc[r][4 * q + 2] = v.z; Wc[r][4 * q + 3] = v.w; }
     }
     // g_i = lam_i + (target_i - u_i) / W_ii is the UNCLAMPED Gauss-Seidel candidate of row i.  A row update
     // lam_j <- clamp(g_j) changes g_i (i != j) by -(W_ij / W_ii) * dlam_j and leaves g_j itself unchanged, so the sweep
@@ -655,112 +645,21 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
       for (int q = 0; q < 3; q++) {
         const P4<T> iv = *reinterpret_cast<const P4<T>*>(vecs + 4 * q), uv = *reinterpret_cast<const P4<T>*>(vecs + 12 + 4 * q);
         const P4<T> tv = *reinterpret_cast<const P4<T>*>(vecs + 24 + 4 * q), lv = *reinterpret_cast<const P4<T>*>(vecs + 36 + 4 * q);
-        g2[2 * q] = p2mk((tv.x - uv.x) * iv.x, (tv.y - uv.y) * iv.y); g2[2 * q + 1] = p2mk((tv.z - uv.z) * iv.z, (tv.w - uv.w) * iv.w);
+        g[4 * q] = (tv.x - uv.x) * iv.x; g[4 * q + 1] = (tv.y - uv.y) * iv.y; g[4 * q + 2] = (tv.z - uv.z) * iv.z; g[4 * q + 3] = (tv.w - uv.w) * iv.w;
         lam[4 * q] = lv.x; lam[4 * q + 1] = lv.y; lam[4 * q + 2] = lv.z; lam[4 * q + 3] = lv.w;
       }
 #pragma unroll
       for (int f = 0; f < 4; f++) lw[f] = lam[3 * f];
 #pragma unroll
-      for (int p = 0; p < 6; p++) {
+      for (int i = 0; i < 12; i++) {
 #pragma unroll
-        for (int f = 0; f < 4; f++) g2[p] = p2fma(Wc[3 * f][p], p2s(-lw[f]), g2[p]);
-        const int i0 = 2 * p, i1 = 2 * p + 1;
-        if (i0 % 3 == 0 && !(actf[i0 / 3] > T(0))) g2[p].x = T(-1e30);
-        if (i1 % 3 == 0 && !(actf[i1 / 3] > T(0))) g2[p].y = T(-1e30);
+        for (int f = 0; f < 4; f++) g[i] = m_fma(Wc[3 * f][i], -lw[f], g[i]);
+        if (i % 3 == 0 && !(actf[i / 3] > T(0))) g[i] = T(-1e30);
       }
     }
     // third barrier of the substep: every lane's loads of the exchange area are done before any lane's next substep stores into it
     // (measured: alternating between two areas instead costs 10 % — more shared memory per CTA and parity-dependent addressing)
     cm.sync();
-  }
-  } else {
-  // float64 validation build: the fully redundant build (every lane gathers all rows with 4-lane broadcasts and forms the whole matrix);
-  // the shared-memory exchange above is the f32 choice; in f64 it moves twice the shared-memory traffic next to a saturated FP64 pipe,
-  // so the f64 build keeps this shuffle-only variant
-  // --- gather every foot's rows on every lane (4-lane broadcasts), then the whole 12x12 contact problem is solved
-  //     REDUNDANTLY in registers by all four lanes: the Gauss-Seidel sweep below has no shuffle on its dependent chain.
-  //     Row index r = 3*foot + e (e: 0 normal, 1,2 friction).
-  T Ya[12][6], Wd[4][6], u0[12], targn[4], actf[4];
-#pragma unroll
-  for (int f = 0; f < 4; f++) {
-#pragma unroll
-    for (int e = 0; e < 3; e++) {
-#pragma unroll
-      for (int c = 0; c < 6; c++) Ya[3 * f + e][c] = cm.bcast(Y[e][c], f);
-      u0[3 * f + e] = cm.bcast(u[e], f);
-    }
-    Wd[f][0] = cm.bcast(Wl[0][0], f); Wd[f][1] = cm.bcast(Wl[1][0], f); Wd[f][2] = cm.bcast(Wl[1][1], f);
-    Wd[f][3] = cm.bcast(Wl[2][0], f); Wd[f][4] = cm.bcast(Wl[2][1], f); Wd[f][5] = cm.bcast(Wl[2][2], f);
-    targn[f] = cm.bcast(dist > T(0) ? -dist * idt : cf.erp * (-dist) * idt, f);
-    actf[f] = cm.bcast(act ? T(1) : T(0), f);
-    lam[3 * f] = cm.bcast(act ? cf.warm * s.lam_n : T(0), f);   // warm start of the normal impulse (Bullet 0.85)
-    lam[3 * f + 1] = T(0); lam[3 * f + 2] = T(0);
-  }
-  // Delassus matrix W = J M^-1 J^T (symmetric): W_ij = Y_i . Y_j (+ the leg-local 3x3 block on the diagonal blocks), built
-  // directly in the layout the sweep consumes — PAIRS of adjacent rows, scalar broadcast operand: WR[r][p] = (W[2p][r], W[2p+1][r]).
-  // Only the pairs at or below the diagonal are computed (42 x 6 pair FMAs instead of 78 x 6 for the full matrix); the rest are
-  // re-paired from them by symmetry.  The substep body is straight-line code, so instruction count is what matters.
-  P2<T> WR[12][6];
-  {
-    P2<T> YP[6][6];
-#pragma unroll
-    for (int p = 0; p < 6; p++) {
-#pragma unroll
-      for (int c = 0; c < 6; c++) YP[p][c] = p2mk(Ya[2 * p][c], Ya[2 * p + 1][c]);
-    }
-#pragma unroll
-    for (int r = 0; r < 12; r++) {
-#pragma unroll
-      for (int p = 0; p <= r / 2; p++) {
-        P2<T> acc = p2mul(YP[p][0], p2s(Ya[r][0]));
-#pragma unroll
-        for (int c = 1; c < 6; c++) acc = p2fma(YP[p][c], p2s(Ya[r][c]), acc);
-        const int f = r / 3, a = r % 3;
-        if ((2 * p) / 3 == f) { const int bb = (2 * p) % 3; acc.x += Wd[f][a >= bb ? a * (a + 1) / 2 + bb : bb * (bb + 1) / 2 + a]; }
-        if ((2 * p + 1) / 3 == f) { const int bb = (2 * p + 1) % 3; acc.y += Wd[f][a >= bb ? a * (a + 1) / 2 + bb : bb * (bb + 1) / 2 + a]; }
-        WR[r][p] = acc;
-      }
-    }
-#pragma unroll
-    for (int r = 0; r < 12; r++) {
-#pragma unroll
-      for (int p = r / 2 + 1; p < 6; p++) {   // rows 2p, 2p+1 > r: W[2p][r] = W[r][2p] lives in WR[2p][r/2]
-        WR[r][p].x = (r & 1) ? WR[2 * p][r / 2].y : WR[2 * p][r / 2].x;
-        WR[r][p].y = (r & 1) ? WR[2 * p + 1][r / 2].y : WR[2 * p + 1][r / 2].x;
-      }
-    }
-  }
-  // g_i = lam_i + (target_i - u_i) / W_ii is the UNCLAMPED Gauss-Seidel candidate of row i.  A row update
-  // lam_j <- clamp(g_j) changes g_i (i != j) by -(W_ij / W_ii) * dlam_j and leaves g_j itself unchanged, so the sweep
-  // carries g instead of the contact velocities.  Inactive feet: zero scale (g frozen), g_n = -BIG => lam stays 0.
-  // Wc[r][p] = (W'[2p][r], W'[2p+1][r]), W'_ij = W_ij / W_ii with a zero diagonal
-  {
-    P2<T> invd[6], uu[6];
-#pragma unroll
-    for (int p = 0; p < 6; p++) {
-      const int i0 = 2 * p, i1 = 2 * p + 1;
-      T d0 = (i0 & 1) ? WR[i0][i0 / 2].y : WR[i0][i0 / 2].x, d1 = (i1 & 1) ? WR[i1][i1 / 2].y : WR[i1][i1 / 2].x;
-      invd[p].x = actf[i0 / 3] > T(0) ? m_rcp(d0) : T(0);
-      invd[p].y = actf[i1 / 3] > T(0) ? m_rcp(d1) : T(0);
-      uu[p] = p2mk(u0[i0], u0[i1]);
-#pragma unroll
-      for (int f = 0; f < 4; f++) uu[p] = p2fma(WR[3 * f][p], p2s(lam[3 * f]), uu[p]);
-      P2<T> tg = p2mk((i0 % 3 == 0) ? targn[i0 / 3] : T(0), (i1 % 3 == 0) ? targn[i1 / 3] : T(0));
-      P2<T> res = p2mk(tg.x - uu[p].x, tg.y - uu[p].y);
-      g2[p] = p2fma(res, invd[p], p2mk(lam[i0], lam[i1]));
-      if (i0 % 3 == 0 && !(actf[i0 / 3] > T(0))) g2[p].x = T(-1e30);
-      if (i1 % 3 == 0 && !(actf[i1 / 3] > T(0))) g2[p].y = T(-1e30);
-    }
-#pragma unroll
-    for (int r = 0; r < 12; r++) {
-#pragma unroll
-      for (int p = 0; p < 6; p++) {
-        Wc[r][p] = p2mul(WR[r][p], invd[p]);
-        if (2 * p == r) Wc[r][p].x = T(0);
-        if (2 * p + 1 == r) Wc[r][p].y = T(0);
-      }
-    }
-  }
   }
   // --- projected Gauss-Seidel, Bullet row order: normals of feet 0..3, then (t1,t2) of feet 0..3.
   //     Row update = clamp -> delta -> 11 independent scalar FFMAs (W'_rr = 0: the row's own candidate is unchanged).
@@ -768,29 +667,23 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
 #pragma unroll
     for (int f = 0; f < 4; f++) {
       const int r = 3 * f;
-      T gr = (r & 1) ? g2[r >> 1].y : g2[r >> 1].x;
-      T ln = m_max(gr, T(0));
+      T ln = m_max(g[r], T(0));
       T dl = lam[r] - ln; lam[r] = ln;          // dl = -(delta lambda)
 #pragma unroll
-      for (int p = 0; p < 6; p++) {
-        if (2 * p != r) g2[p].x = m_fma(Wc[r][p].x, dl, g2[p].x);
-        if (2 * p + 1 != r) g2[p].y = m_fma(Wc[r][p].y, dl, g2[p].y);
-      }
+      for (int i = 0; i < 12; i++)
+        if (i != r) g[i] = m_fma(Wc[r][i], dl, g[i]);
     }
 #pragma unroll
     for (int f = 0; f < 4; f++) {
 #pragma unroll
       for (int td = 1; td < 3; td++) {
         const int r = 3 * f + td;
-        T gr = (r & 1) ? g2[r >> 1].y : g2[r >> 1].x;
         T lim = pr.mu * lam[3 * f];
-        T ln = m_min(m_max(gr, -lim), lim);
+        T ln = m_min(m_max(g[r], -lim), lim);
         T dl = lam[r] - ln; lam[r] = ln;
 #pragma unroll
-        for (int p = 0; p < 6; p++) {
-          if (2 * p != r) g2[p].x = m_fma(Wc[r][p].x, dl, g2[p].x);
-          if (2 * p + 1 != r) g2[p].y = m_fma(Wc[r][p].y, dl, g2[p].y);
-        }
+        for (int i = 0; i < 12; i++)
+          if (i != r) g[i] = m_fma(Wc[r][i], dl, g[i]);
       }
     }
   }

@@ -53,8 +53,6 @@ struct HostComm {
     x->bar.wait();
     return r;
   }
-  T xor1(T v) const { x->A[k] = (double)v; x->bar.wait(); T r = (T)x->A[k ^ 1]; x->bar.wait(); return r; }
-  T xor2(T v) const { x->A[k] = (double)v; x->bar.wait(); T r = (T)x->A[k ^ 2]; x->bar.wait(); return r; }
   T bcast(T v, int f) const {
     x->A[k] = (double)v; x->bar.wait();
     T r = (T)x->A[f];
