@@ -60,6 +60,16 @@ for _ in range(2):
     g2.learn(*rpm.sample_batch(256, out=g2.static_batch()), graph=True, pull=False)
 expert = MujocoAgent(49, 12, seed=2)
 learner.bc_learn(torch.randn(256, 49, device="cuda"), torch.randn(256, 49, device="cuda"), expert)
+# a non-default learner (A = 1: the runtime-dimension actor head, 32-thread dy blocks, one tile) and a full-width (in_dim 64) MLP on a
+# partial last tile
+small = SACLearner(MujocoAgent(3, 1, seed=3), 128)
+small.learn(torch.randn(128, 3, device="cuda"), torch.rand(128, 1, device="cuda") * 2 - 1, torch.randn(128, device="cuda"), torch.randn(128, 3, device="cuda"), torch.ones(128, device="cuda"))
+from paddlerobotics_b200.agent import FusedMLP
+wide = FusedMLP(64, 2, 2)
+for i in range(2):
+    wide.set_weights(i, torch.randn(256, 64, device="cuda") * 0.1, torch.zeros(256, device="cuda"), torch.randn(256, 256, device="cuda") * 0.05,
+                     torch.zeros(256, device="cuda"), torch.randn(2, 256, device="cuda") * 0.05, torch.zeros(2, device="cuda"))
+wide.forward(torch.randn(129, 52, device="cuda"), in2=torch.randn(129, 12, device="cuda"), mode=1, seed=5)
 ev = PopulationEvaluator(4, 2, max_steps=5)
 ev.evaluate(np.repeat(w[None], 4, 0), np.repeat(b[None], 4, 0))
 torch.cuda.synchronize()
