@@ -107,7 +107,11 @@ B2Q_HD T terrain_height(const Cfg<T>& cf, T x, T y, V3<T>& n) {
   T fx = (x - cf.hf_x0) * cf.hf_icell, fy = (y - cf.hf_y0) * cf.hf_icell;
   fx = m_min(m_max(fx, T(0)), T(cf.hf_nx) - T(1.000001));
   fy = m_min(m_max(fy, T(0)), T(cf.hf_ny) - T(1.000001));
+  // In float32 nx - 1.000001 rounds to nx - 1 once nx >= ~17, so the cell index is clamped as an integer too: at or past the far
+  // edge the lookup stays in the last cell (tx or ty = 1) and never reads column nx or the row past the end of the field.
   int ix = (int)fx, iy = (int)fy;
+  if (ix > cf.hf_nx - 2) ix = cf.hf_nx - 2;
+  if (iy > cf.hf_ny - 2) iy = cf.hf_ny - 2;
   T tx = fx - T(ix), ty = fy - T(iy);
   const T* h = cf.hf; int nx = cf.hf_nx;
   T h00 = h[iy * nx + ix], h10 = h[iy * nx + ix + 1], h01 = h[(iy + 1) * nx + ix], h11 = h[(iy + 1) * nx + ix + 1];

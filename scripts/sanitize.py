@@ -21,7 +21,10 @@ for kw in (dict(num_envs=13), dict(num_envs=16, precision="f64"), dict(num_envs=
            # memory, TORQUE mode, base push, damping) in f32 and f64
            dict(num_envs=13, sensor_motor=2, sensor_imu=2, obs_normal=0, noise_stdev=(0.01, 0.05, 0.1, 0.02, 0.04), stuck_termination=1, body_collisions=1, auto_reset=True),
            dict(num_envs=11, joint_limits=1, knee_contacts=1, external_force=1, base_damping=(0.04, 0.02, 0.04, 0.01)), dict(num_envs=9, joint_limits=1, precision="f64"),
-           dict(num_envs=8, motor_mode=1), dict(num_envs=8, motor_mode=2)):
+           dict(num_envs=8, motor_mode=1), dict(num_envs=8, motor_mode=2),
+           # height-field far edges: the field ends 0.35 m behind the robot in x and y, so every foot lies beyond both far edges (the
+           # cell index is clamped to nx - 2 / ny - 2; in f32, nx - 1.000001 rounds to nx - 1)
+           dict(num_envs=13, heightfield=(hf[:24, :24], -1.5, -1.5, 0.05)), dict(num_envs=13, heightfield=(hf[:24, :24], -1.5, -1.5, 0.05), precision="f64")):
     env = VecQuadrupedalEnv(**kw)
     n = env.num_envs
     env.reset(w, b)

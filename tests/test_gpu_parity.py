@@ -519,7 +519,8 @@ def test_large_batch_and_error_paths(torch_cuda, etg_default):
 @pytest.mark.parametrize("n", [13, 64])
 def test_step_host_io_modes_identical(torch_cuda, etg_stable, n, monkeypatch):
     """b2q_step_host: zero-copy pinned buffers (B2Q_HOST_IO=2, default), zero-copy actions only (1), memcpy staging (0) and
-    PAGEABLE numpy buffers all return bit-identical obs / reward / done / info; n=13 exercises the ragged last CTA."""
+    PAGEABLE numpy buffers all return bit-identical obs / reward / done / info (the zero-copy info rows are their own store path);
+    n=13 exercises the ragged last CTA."""
     import ctypes as C
     from paddlerobotics_b200.env import VecQuadrupedalEnv
     w, b = etg_stable
@@ -538,10 +539,10 @@ def test_step_host_io_modes_identical(torch_cuda, etg_stable, n, monkeypatch):
                                            d.ctypes.data_as(C.c_void_p), inf.ctypes.data_as(C.c_void_p), None)
                 assert rc == 0
             else:
-                o, r, d = env.step_host(a)
-            outs.append((o.copy(), r.copy(), d.copy()))
+                o, r, d, inf = env.step_host(a, info=True)
+            outs.append((o.copy(), r.copy(), d.copy(), inf.copy()))
         results.append(outs)
         env.close()
     for other in results[1:]:
-        for (o0, r0, d0), (o1, r1, d1) in zip(results[0], other):
-            assert np.array_equal(o0, o1) and np.array_equal(r0, r1) and np.array_equal(d0, d1)
+        for (o0, r0, d0, i0), (o1, r1, d1, i1) in zip(results[0], other):
+            assert np.array_equal(o0, o1) and np.array_equal(r0, r1) and np.array_equal(d0, d1) and np.array_equal(i0, i1)
