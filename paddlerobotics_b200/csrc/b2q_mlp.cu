@@ -341,33 +341,12 @@ __global__ void __launch_bounds__(NTHR, 1) b2q_mlp_fwd_kernel(FwdArgs a) { pdl_s
   }
 }
 
-// f32 nn.Linear weights -> bf16 swizzled operand images (+ f32 biases) in the per-net image
-__global__ void b2q_mlp_pack_kernel(uint8_t* img, const float* w1, const float* b1, const float* w2, const float* b2, const float* w3, const float* b3,
-                                    int in_dim, int out_dim, int a_off, int a_dim) { pdl_sync();
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < HID * HID) {   // W2^T image: B operand [N = in][K = out] of the input-gradient pass
-    int n = i >> 8, k = i & 255;
-    *reinterpret_cast<__nv_bfloat16*>(img + IMG_W2T + sw128_offset(n, k, HID)) = __float2bfloat16(w2[(size_t)k * HID + n]);
-  }
-  if (i < 16 * HID) {    // W1A image: [N = 16 action slots][K = hidden]
-    int n = i >> 8, k = i & 255;
-    *reinterpret_cast<__nv_bfloat16*>(img + IMG_W1A + sw128_offset(n, k, 16)) = __float2bfloat16(n < a_dim ? w1[(size_t)k * in_dim + a_off + n] : 0.f);
-  }
-  if (i < HID * 64) {  // W1 [256 x 64 padded]
-    int n = i >> 6, k = i & 63;
-    *reinterpret_cast<__nv_bfloat16*>(img + IMG_W1 + sw128_offset(n, k, HID)) = __float2bfloat16(k < in_dim ? w1[(size_t)n * in_dim + k] : 0.f);
-  }
-  if (i < HID * HID) {
-    int n = i >> 8, k = i & 255;
-    *reinterpret_cast<__nv_bfloat16*>(img + IMG_W2 + sw128_offset(n, k, HID)) = __float2bfloat16(w2[(size_t)n * HID + k]);
-  }
-  if (i < 32 * HID) {
-    int n = i >> 8, k = i & 255;
-    *reinterpret_cast<__nv_bfloat16*>(img + IMG_W3 + sw128_offset(n, k, 32)) = __float2bfloat16(n < out_dim ? w3[(size_t)n * HID + k] : 0.f);
-  }
-  float* bias = reinterpret_cast<float*>(img + IMG_BIAS);
-  if (i < HID) { bias[i] = b1[i]; bias[HID + i] = b2[i]; }
-  if (i < 32) bias[2 * HID + i] = i < out_dim ? b3[i] : 0.f;
+// f32 nn.Linear weights -> one net's image: a thread per parameter, in the flat order the packer indexes
+__global__ void b2q_mlp_pack_kernel(PackDst d, const float* w1, const float* b1, const float* w2, const float* b2, const float* w3, const float* b3) { pdl_sync();
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= d.n) return;
+  const float v = i < d.ob1 ? w1[i] : i < d.oW2 ? b1[i - d.ob1] : i < d.ob2 ? w2[i - d.oW2] : i < d.oW3 ? b2[i - d.ob2] : i < d.ob3 ? w3[i - d.oW3] : b3[i - d.ob3];
+  pack_param(d, i, v);
 }
 
 }  // namespace
@@ -415,7 +394,8 @@ uint8_t* b2q_mlp_image(B2QMlpHandle h, int net) { return (h && net >= 0 && net <
 
 int b2q_mlp_set_weights(B2QMlpHandle h, int net, const float* w1, const float* b1, const float* w2, const float* b2, const float* w3, const float* b3, void* stream) {
   if (!h || net < 0 || net >= h->nets || !w1 || !b1 || !w2 || !b2 || !w3 || !b3) { if (h) h->err = "b2q_mlp_set_weights: bad argument"; return -1; }
-  pdl_launch(b2q_mlp_pack_kernel, dim3((HID * HID + 255) / 256), dim3(256), 0, (cudaStream_t)stream, h->img + (size_t)net * IMG_BYTES, w1, b1, w2, b2, w3, b3, h->in_dim, h->out_dim, h->a_off, h->a_dim);
+  const PackDst d = pack_dst(h->img + (size_t)net * IMG_BYTES, h->in_dim, h->out_dim, h->a_off, h->a_dim);
+  pdl_launch(b2q_mlp_pack_kernel, dim3((d.n + 255) / 256), dim3(256), 0, (cudaStream_t)stream, d, w1, b1, w2, b2, w3, b3);
   h->launches++;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return -2; }

@@ -9,7 +9,6 @@
 // bf16 copy refreshed by the optimiser kernel.
 #include <cuda.h>
 #include <cuda_runtime.h>
-#include <cstdlib>
 #include <map>
 #include <tuple>
 #include <cuda_bf16.h>
@@ -49,6 +48,7 @@ struct GemmArgs {
 constexpr int G_NSTAGE = 4;
 constexpr uint32_t G_STAGE_A = 128 * 128, G_STAGE_B = 64 * 128, G_STAGE = G_STAGE_A + G_STAGE_B;   // bytes: 128 x 64 bf16 and BN(<=64) x 64 bf16
 constexpr uint32_t G_SMEM = G_NSTAGE * G_STAGE + 128 + 1024;                                       // + barriers + alignment slack
+constexpr int B2Q_GEMM_SPLIT_DIV = 8;                                                               // K chunks (of 64) per split-K CTA
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, uint32_t bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
@@ -175,14 +175,6 @@ __global__ void __launch_bounds__(128) b2q_gemm_kernel(const __grid_constant__ C
 
 // ---------------------------------------------------------------------------------------------------------------------
 // elementwise / reduction kernels
-// critic head backward for both nets: dq = 2 (q - tq)/B; loss += (q-tq)^2/B; db3 += dq   (mse_loss mean reduction, sac.py:94-95)
-__global__ void k_critic_dq(const float* q /*[2][B]*/, const float* tq /*[B] or [2][B]*/, int tq_stride, float* dq /*[2][B]*/, float* loss, int B) { pdl_sync();
-  int b = blockIdx.x * blockDim.x + threadIdx.x, net = blockIdx.y;
-  float l = 0.f;
-  if (b < B) { float e = q[net * B + b] - tq[net * tq_stride + b]; dq[net * B + b] = 2.f * e / (float)B; l = e * e / (float)B; }
-  for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
-  if ((threadIdx.x & 31) == 0) atomicAdd(loss, l);
-}
 // Vectorised tile kernels: a block walks SUBT sub-tiles of 32 batch rows x 256 hidden columns (256 threads: a warp handles one row at a
 // time, each lane 8 consecutive columns — 16-byte bf16 / 2 x 16-byte f32 accesses, fully coalesced).  Column sums and the head's weight
 // gradient are accumulated in registers / shared memory over the block's SUBT x 32 rows and flushed with ONE atomic per column per block
@@ -202,18 +194,18 @@ __device__ __forceinline__ void colsum_flush(float (*csum)[H], const float* cs /
   __syncthreads();
 }
 // critic head backward (out_dim = 1), same tiling: dh2[b,:] = dq[b] W3 masked by h2 > 0; dW3 += sum_b dq[b] h2[b,:]; db3 += sum_b dq; db2 += sum_b dh2
-// How a row's dq is obtained: from an array, or computed in place so that the tiny dq kernels drop out of the dependency chain
-//   DQ_CRITIC: dq = 2 (q - tq)/B with tq = r + gamma * term * (min(q1', q2') - alpha * logp')  (sac.py:85-95; loss += (q - tq)^2 / B)
-enum { DQ_ARRAY = 0, DQ_CRITIC = 1 };
+// A row's dq = 2 (q - tq)/B is computed in place (mse_loss mean reduction, loss += (q - tq)^2 / B), so no dq kernel sits on the dependency chain:
+//   DQ_CRITIC: tq = r + gamma * term * (min(q1', q2') - alpha * logp')  (sac.py:85-95)
+//   DQ_TWIN:   tq = qn[net][b], the expert's twin Q (BC.py:63-67)
+enum { DQ_CRITIC = 0, DQ_TWIN = 1 };
 struct DqSrc { int mode, net; const float *q /*[2][B]*/, *rew, *term, *qn /*[2][B]*/, *logpn; float gamma, alpha; float* loss; };
-__device__ __forceinline__ float dq_of_row(const DqSrc& d, const float* dq, int b, int B, float& loss_acc) {
-  if (d.mode == DQ_ARRAY) return dq[b];
-  const float tq = d.rew[b] + d.gamma * d.term[b] * (fminf(d.qn[b], d.qn[B + b]) - d.alpha * d.logpn[b]);
+__device__ __forceinline__ float dq_of_row(const DqSrc& d, int b, int B, float& loss_acc) {
+  const float tq = d.mode == DQ_TWIN ? d.qn[d.net * B + b] : d.rew[b] + d.gamma * d.term[b] * (fminf(d.qn[b], d.qn[B + b]) - d.alpha * d.logpn[b]);
   const float e = d.q[d.net * B + b] - tq;
   loss_acc += e * e / (float)B;
   return 2.f * e / (float)B;
 }
-__global__ void __launch_bounds__(256) k_head_bwd1(const float* __restrict__ dq /*[B]*/, DqSrc src, const float* __restrict__ W3 /*[256]*/, const bf16* __restrict__ h2,
+__global__ void __launch_bounds__(256) k_head_bwd1(DqSrc src, const float* __restrict__ W3 /*[256]*/, const bf16* __restrict__ h2,
                                                    bf16* __restrict__ dh_rm, bf16* __restrict__ dh_t, float* dW3 /*[256]*/, float* db3 /*[1] or null*/, float* db2 /*[256] or null*/, int B) { pdl_sync();
   __shared__ __align__(16) bf16 tile[32][H + 8];
   __shared__ float csum[8][H];
@@ -229,7 +221,7 @@ __global__ void __launch_bounds__(256) k_head_bwd1(const float* __restrict__ dq 
 #pragma unroll
     for (int k = 0; k < 4; k++) {
       const int r = warp + 8 * k;
-      if (r < nr) { hv[k] = *reinterpret_cast<const uint4*>(h2 + (size_t)(b0 + r) * H + chunk * 8); d[k] = dq_of_row(src, dq, b0 + r, B, sloss); } else d[k] = 0.f;
+      if (r < nr) { hv[k] = *reinterpret_cast<const uint4*>(h2 + (size_t)(b0 + r) * H + chunk * 8); d[k] = dq_of_row(src, b0 + r, B, sloss); } else d[k] = 0.f;
     }
 #pragma unroll
     for (int k = 0; k < 4; k++) {
@@ -253,7 +245,7 @@ __global__ void __launch_bounds__(256) k_head_bwd1(const float* __restrict__ dq 
   }
   colsum_flush(csum, acc, chunk, warp, dW3);                 // dW3: per-thread partials reduced over the 8 warps, one atomic per column
   if (db3 && chunk == 0) atomicAdd(db3, sdq);               // every lane of a warp holds the same rows: one lane per warp adds its dq sum
-  if (src.mode == DQ_CRITIC && chunk == 0) atomicAdd(src.loss, sloss);   // ... and its share of the critic loss
+  if (chunk == 0) atomicAdd(src.loss, sloss);               // ... and its share of the critic loss
   colsum_flush(csum, cs, chunk, warp, db2);
 }
 // The head gradient dy = dloss/d[mean | raw_ls] leaves the dy kernels as bf16 in the two operand layouts the tensor-core GEMMs read
@@ -310,51 +302,13 @@ __global__ void __launch_bounds__(384) k_bc_dy(const float* raw /*[B][2A]*/, con
   sT[j][r] = __float2bfloat16(g0); sT[A + j][r] = __float2bfloat16(g1);
   dy_store_block(sT, l, b0, B, A, dy_rm, dy_t, db3, loss);
 }
-// Adam (torch.optim.Adam defaults: betas 0.9/0.999, eps 1e-8, no weight decay), sac.py:55-58
-__global__ void k_step_inc(int* step) { pdl_sync(); *step += 1; }
-// the step counter lives on the device so that the whole learn() can be replayed from a CUDA graph
-// `step` holds the number of COMPLETED optimiser steps; both Adam kernels of a learn use step + 1 and the last kernel of the learn
-// (k_adam_pack's last block / k_step_inc) advances it — no separate increment kernel in front of the Adam on the dependency chain
-__global__ void k_adam(float* p, const float* g, float* m, float* v, int n, float lr, float b1, float b2, float eps, const int* step) { pdl_sync();
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    const float t = (float)(*step + 1), bc1 = 1.f - powf(b1, t), bc2 = 1.f - powf(b2, t);
-    float gi = g[i], mi = b1 * m[i] + (1.f - b1) * gi, vi = b2 * v[i] + (1.f - b2) * gi * gi;
-    m[i] = mi; v[i] = vi;
-    p[i] -= lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);
-  }
-}
-// The optimiser kernels below also REPACK what they update: each thread converts its new parameter to bf16 and stores it where the tensor-core
-// kernels read it — the forward image of its net (K-major SWIZZLE_128B operand images + f32 biases, b2q_mlp_internal.h) and the backward copies
-// (W2^T, W3^T padded to 64, the action columns of W1) — so no pack / copy kernel follows an optimiser step on the dependency chain.
-// Padding entries of the images are zero from allocation and never change.
-struct PackDst { uint8_t* img; bf16 *W2T, *W3T, *W1A; int in_dim, od, a_off, a_dim, gradin /*also keep the W2^T / W1A operand images of the input-gradient pass*/; unsigned oW1, ob1, oW2, ob2, oW3, ob3, n; };
-struct PackDst2 { PackDst d[2]; };
-__device__ __forceinline__ void pack_one(const PackDst& d, unsigned i, float v) {
-  const bf16 vb = __float2bfloat16(v);
-  float* bias = reinterpret_cast<float*>(d.img + b2q_mlp_img::IMG_BIAS);
-  if (i < d.ob1) {                                   // W1 [256][in_dim]
-    const int n = (int)(i / (unsigned)d.in_dim), k = (int)i - n * d.in_dim;
-    *reinterpret_cast<bf16*>(d.img + b2q_mlp_img::IMG_W1 + sw128_offset(n, k, H)) = vb;
-    if (d.W1A && k >= d.a_off && k < d.a_off + d.a_dim) {
-      d.W1A[(size_t)(k - d.a_off) * H + n] = vb;
-      if (d.gradin) *reinterpret_cast<bf16*>(d.img + b2q_mlp_img::IMG_W1A + sw128_offset(k - d.a_off, n, 16)) = vb;
-    }
-  } else if (i < d.oW2) { bias[i - d.ob1] = v;
-  } else if (i < d.ob2) {                            // W2 [256][256]
-    const int j = (int)(i - d.oW2), n = j >> 8, k = j & 255;
-    *reinterpret_cast<bf16*>(d.img + b2q_mlp_img::IMG_W2 + sw128_offset(n, k, H)) = vb;
-    if (d.W2T) d.W2T[(size_t)k * H + n] = vb;
-    if (d.gradin) *reinterpret_cast<bf16*>(d.img + b2q_mlp_img::IMG_W2T + sw128_offset(k, n, H)) = vb;
-  } else if (i < d.oW3) { bias[H + i - d.ob2] = v;
-  } else if (i < d.ob3) {                            // W3 [od][256]
-    const int j = (int)(i - d.oW3), n = j >> 8, k = j & 255;
-    *reinterpret_cast<bf16*>(d.img + b2q_mlp_img::IMG_W3 + sw128_offset(n, k, 32)) = vb;
-    if (d.W3T) d.W3T[(size_t)k * 64 + n] = vb;
-  } else { bias[2 * H + i - d.ob3] = v; }
-}
-// Adam over `nets` consecutive parameter blocks of dst.d[0].n floats each + repack.  `ticket` (optional): the last block to finish advances the
-// step counter, so the kernel can close a learn step while another stream runs the Polyak update beside it.
+// The optimiser kernels also REPACK what they update: each thread stores its new parameter through pack_param (b2q_mlp_internal.h) where the
+// tensor-core kernels read it — the forward image of its net and the bf16 backward copies — so no pack kernel follows an optimiser step on the
+// dependency chain.  k_pack does the same for parameters set from outside.
+// Adam (torch.optim.Adam defaults: betas 0.9/0.999, eps 1e-8, no weight decay), sac.py:55-58, over the parameter blocks of one or two nets.
+// The step counter lives on the device so that the whole learn() can be replayed from a CUDA graph.  `step` holds the number of COMPLETED
+// optimiser steps: both Adam kernels of a learn use step + 1, and the one given `ticket` closes the step — its last block to finish advances
+// the counter, so no increment kernel sits on the dependency chain and the kernel can run while another stream runs the Polyak update beside it.
 __global__ void __launch_bounds__(256) k_adam_pack(float* p, const float* g, float* m, float* v, int n, float lr, float b1, float b2, float eps, int* step, int* ticket, PackDst2 dst) { pdl_sync();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
@@ -364,7 +318,7 @@ __global__ void __launch_bounds__(256) k_adam_pack(float* p, const float* g, flo
     const float pn = p[i] - lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);
     p[i] = pn;
     const unsigned per = dst.d[0].n, net = (unsigned)i / per;
-    pack_one(dst.d[net], (unsigned)i - net * per, pn);
+    pack_param(dst.d[net], (unsigned)i - net * per, pn);
   }
   if (ticket) {
     __syncthreads();                                  // every thread of the block has read *step
@@ -380,16 +334,15 @@ __global__ void __launch_bounds__(256) k_polyak_pack(float* tgt, const float* sr
     const float tn = tau * src[i] + (1.f - tau) * tgt[i];
     tgt[i] = tn;
     const unsigned per = dst.d[0].n, net = (unsigned)i / per;
-    pack_one(dst.d[net], (unsigned)i - net * per, tn);
+    pack_param(dst.d[net], (unsigned)i - net * per, tn);
   }
 }
-// bf16 helper copies of one net's weights for the backward GEMMs: W2T [256][256], W3T64 [256][64] (k = output index, zero padded),
-// W1A [16][256] (rows = action columns of W1, for d/da)
-__global__ void k_make_bwd_weights(const float* W1, int in_dim, int a_off, int a_dim, const float* W2, const float* W3, int od, bf16* W2T, bf16* W3T, bf16* W1A) { pdl_sync();
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < H * H) { int n = i / H, k = i % H; W2T[i] = __float2bfloat16(W2[(size_t)k * H + n]); }
-  if (i < H * 64) { int n = i / 64, k = i % 64; W3T[i] = __float2bfloat16(k < od ? W3[(size_t)k * H + n] : 0.f); }
-  if (i < 16 * H) { int n = i / H, k = i % H; W1A[i] = __float2bfloat16((a_dim > 0 && n < a_dim) ? W1[(size_t)k * in_dim + a_off + n] : 0.f); }
+__global__ void __launch_bounds__(256) k_pack(const float* p, int n, PackDst2 dst) { pdl_sync();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) {
+    const unsigned per = dst.d[0].n, net = (unsigned)i / per;
+    pack_param(dst.d[net], (unsigned)i - net * per, p[i]);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -418,7 +371,7 @@ struct B2QSac {
   cudaStream_t side = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   cudaStream_t aux[2] = {nullptr, nullptr}; cudaEvent_t ev_aux[4] = {nullptr, nullptr, nullptr, nullptr};   // per-chain helper streams: dW2 GEMM beside the dh1 -> dW1 chain
   bf16 *dh1_rm[2] = {nullptr, nullptr}, *dh1_t[2] = {nullptr, nullptr};                                      // layer-1 gradients (separate from dh2 so both GEMM branches can run)
-  float *q = nullptr, *qn = nullptr, *dq = nullptr, *next_a = nullptr, *next_logp = nullptr, *cur_a = nullptr, *cur_logp = nullptr, *raw_a = nullptr,
+  float *q = nullptr, *qn = nullptr, *next_a = nullptr, *next_logp = nullptr, *cur_a = nullptr, *cur_logp = nullptr, *raw_a = nullptr,
         *da_c = nullptr, *losses = nullptr;
   std::vector<void*> allocs;
   void* tmap_cache = nullptr;   // TmapCache*: TMA tensor maps of the GEMM operands
@@ -481,8 +434,7 @@ int gemm(B2QSac* s, cudaStream_t st, const bf16* A, int lda, const bf16* Bm, int
   if (g.BN > 64) g.BN = 64;                              // N tiled by 64 (grid.y): more CTAs on these latency-bound shapes, 8 KB B panel per k-chunk
   const int ntiles = (N + g.BN - 1) / g.BN;
   int nk = (K + 63) / 64, splits = 1;
-  static const int split_div = [] { const char* e = std::getenv("B2Q_GEMM_SPLIT_DIV"); int v = e ? std::atoi(e) : 8; return v < 1 ? 1 : v; }();   // K chunks (of 64) per split-K CTA
-  if (splitk) { splits = nk / split_div; if (splits < 1) splits = 1; if (splits > 64) splits = 64; }
+  if (splitk) { splits = nk / B2Q_GEMM_SPLIT_DIV; if (splits < 1) splits = 1; if (splits > 64) splits = 64; }
   g.chunks_per_split = (nk + splits - 1) / splits;
   splits = (nk + g.chunks_per_split - 1) / g.chunks_per_split;
   g.atomic = splits > 1 ? 1 : 0;
@@ -509,37 +461,25 @@ int gemm(B2QSac* s, cudaStream_t st, const bf16* A, int lda, const bf16* Bm, int
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
-// forward images + bf16 backward copies after a parameter change; `which`: bit 0 actor, bit 1 critics, bit 2 target critics.
-// Net 0 / the actor are repacked on the caller's stream, net 1 on the side stream (small independent kernels).
-void sync_net_weights(B2QSac* s, cudaStream_t st, int which = 7) {
-  const Net& a = s->an; const Net& c = s->cn;
-  fork(s, st);
-  // the forward-image pack and the bf16 backward copies of a net are independent: the copies run on a helper stream beside the pack
-  // (one stage of the dependency chain instead of two)
-  cudaEventRecord(s->ev_aux[0], st); cudaStreamWaitEvent(s->aux[0], s->ev_aux[0], 0);
-  if (which & 1) {
-    pdl_launch(k_make_bwd_weights, dim3((H * H + 255) / 256), dim3(256), 0, s->aux[0], s->p_actor + a.oW1, a.in_dim, 0, 0, s->p_actor + a.oW2, s->p_actor + a.oW3, a.od, s->W2T[0], s->W3T[0], s->W1A[0]);
-    b2q_mlp_set_weights(s->mlp_actor, 0, s->p_actor + a.oW1, s->p_actor + a.ob1, s->p_actor + a.oW2, s->p_actor + a.ob2, s->p_actor + a.oW3, s->p_actor + a.ob3, st);
-    s->launches += 2;
-  }
+// Where the packer stores each net of a parameter group: the actor (one net; d[1] repeats d[0]), the critics, or the target critics
+// (forward images only: nothing differentiates through them).
+enum { NETS_ACTOR = 0, NETS_CRITIC = 1, NETS_TARGET = 2 };
+PackDst2 dst_of(const B2QSac* s, int group) {
+  const bool actor = group == NETS_ACTOR, crit = group == NETS_CRITIC;
+  const Net& nt = actor ? s->an : s->cn;
+  const B2QMlpHandle mlp = actor ? s->mlp_actor : crit ? s->mlp_critic : s->mlp_target;
+  PackDst2 r;
   for (int i = 0; i < 2; i++) {
-    cudaStream_t sx = i ? s->side : st;
-    float* p = s->p_critic + (size_t)i * c.n; float* t = s->p_target + (size_t)i * c.n;
-    if (which & 2) {
-      pdl_launch(k_make_bwd_weights, dim3((H * H + 255) / 256), dim3(256), 0, s->aux[0], p + c.oW1, c.in_dim, s->D, s->A, p + c.oW2, p + c.oW3, c.od, s->W2T[1 + i], s->W3T[1 + i], s->W1A[1 + i]);
-      b2q_mlp_set_weights(s->mlp_critic, i, p + c.oW1, p + c.ob1, p + c.oW2, p + c.ob2, p + c.oW3, p + c.ob3, sx);
-      s->launches += 2;
-    }
-    if (which & 4) { b2q_mlp_set_weights(s->mlp_target, i, t + c.oW1, t + c.ob1, t + c.oW2, t + c.ob2, t + c.oW3, t + c.ob3, s->side); s->launches++; }
+    PackDst& d = r.d[i];
+    d = pack_dst(b2q_mlp_image(mlp, actor ? 0 : i), nt.in_dim, nt.od, crit ? s->D : 0, crit ? s->A : 0);
+    if (group != NETS_TARGET) { const int bw = actor ? 0 : 1 + i; d.W2T = s->W2T[bw]; d.W3T = s->W3T[bw]; d.W1A = s->W1A[bw]; }
   }
-  cudaEventRecord(s->ev_aux[1], s->aux[0]); cudaStreamWaitEvent(st, s->ev_aux[1], 0);
-  join(s, st);
+  return r;
 }
 
 }  // namespace
 
 namespace {
-// weight gradients of both critics from dq [2][B] and the activation dumps of the last critic forward
 // one MLP's weight-gradient chain after its head backward: dW2 (split-K GEMM over the batch) runs on the helper stream `ax`
 // beside  dh1 = (dh2 W2) . relu'  ->  dW1  on `st`
 int hidden_backward(B2QSac* s, cudaStream_t st, int slot, const bf16* dh2_rm, const bf16* dh2_t, const bf16* h1_rm, const bf16* h1_t, const bf16* x_t,
@@ -556,8 +496,8 @@ int hidden_backward(B2QSac* s, cudaStream_t st, int slot, const bf16* dh2_rm, co
   s->launches += 3;
   return 0;
 }
-// weight gradients of both critics from dq [2][B] and the activation dumps of the last critic forward
-int critic_backward(B2QSac* s, cudaStream_t st0, DqSrc src = DqSrc{DQ_ARRAY, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, 0.f, nullptr}) {
+// weight gradients of both critics from the dq of `src` and the activation dumps of the last critic forward
+int critic_backward(B2QSac* s, cudaStream_t st0, DqSrc src) {
   const int B = s->B; const Net& cn = s->cn;
   fork(s, st0);
   for (int i = 0; i < 2; i++) {
@@ -566,7 +506,7 @@ int critic_backward(B2QSac* s, cudaStream_t st0, DqSrc src = DqSrc{DQ_ARRAY, 0, 
     float* g = s->g_critic + (size_t)i * cn.n; const float* p = s->p_critic + (size_t)i * cn.n;
     const bf16 *h1 = s->hc1_rm + (size_t)i * B * H, *h1t = s->hc1_t + (size_t)i * B * H, *h2 = s->hc2_rm + (size_t)i * B * H;
     src.net = i;
-    pdl_launch(k_head_bwd1, dim3((B + 32 * SUBT - 1) / (32 * SUBT)), dim3(H), 0, st, s->dq + (size_t)i * B, src, p + cn.oW3, h2, dh_rm, dh_t, g + cn.oW3, g + cn.ob3, g + cn.ob2, B);   // (dq,) dh2, dW3, db3, db2
+    pdl_launch(k_head_bwd1, dim3((B + 32 * SUBT - 1) / (32 * SUBT)), dim3(H), 0, st, src, p + cn.oW3, h2, dh_rm, dh_t, g + cn.oW3, g + cn.ob3, g + cn.ob2, B);   // dh2, dW3, db3, db2
     s->launches++;
     if (hidden_backward(s, st, i, dh_rm, dh_t, h1, h1t, s->xc_t, s->W2T[1 + i], g + cn.oW2, g + cn.ob1, g + cn.oW1, cn.in_dim)) return -2;
   }
@@ -612,7 +552,7 @@ int b2q_sac_create(int device, int obs_dim, int act_dim, int batch, float gamma,
   ok = ok && dalloc(s, &s->xc_t, 64 * Bz) && dalloc(s, &s->hc1_rm, 2 * Bz * H) && dalloc(s, &s->hc1_t, 2 * Bz * H) && dalloc(s, &s->hc2_rm, 2 * Bz * H) &&
        dalloc(s, &s->hc2_t, 2 * Bz * H) && dalloc(s, &s->xa_t, 64 * Bz) && dalloc(s, &s->ha1_rm, Bz * H) && dalloc(s, &s->ha1_t, Bz * H) &&
        dalloc(s, &s->ha2_rm, Bz * H) && dalloc(s, &s->ha2_t, Bz * H) && dalloc(s, &s->dh_rm, Bz * H) && dalloc(s, &s->dh_t, Bz * H) && dalloc(s, &s->dy_bf, Bz * 128) && dalloc(s, &s->dy_rm, Bz * 64) &&
-       dalloc(s, &s->q, 2 * Bz) && dalloc(s, &s->qn, 2 * Bz) && dalloc(s, &s->dq, 2 * Bz) && dalloc(s, &s->next_a, Bz * 12) &&
+       dalloc(s, &s->q, 2 * Bz) && dalloc(s, &s->qn, 2 * Bz) && dalloc(s, &s->next_a, Bz * 12) &&
        dalloc(s, &s->next_logp, Bz) && dalloc(s, &s->cur_a, Bz * 12) && dalloc(s, &s->cur_logp, Bz) && dalloc(s, &s->raw_a, Bz * 24) && dalloc(s, &s->da_c, 2 * Bz * 16) &&
        dalloc(s, &s->losses, 4) && dalloc(s, &s->d_step, 2 /*step | block ticket of the closing Adam*/) &&
        dalloc(s, &s->dh_rm2, Bz * H) && dalloc(s, &s->dh_t2, Bz * H) &&
@@ -658,7 +598,11 @@ int b2q_sac_set_params(B2QSacHandle s, const float* actor, const float* critic, 
   if (critic) cudaMemcpyAsync(s->p_critic, critic, 2 * s->cn.n * sizeof(float), cudaMemcpyDeviceToDevice, st);
   if (target) cudaMemcpyAsync(s->p_target, target, 2 * s->cn.n * sizeof(float), cudaMemcpyDeviceToDevice, st);
   else if (critic) cudaMemcpyAsync(s->p_target, critic, 2 * s->cn.n * sizeof(float), cudaMemcpyDeviceToDevice, st);   // MujocoAgent: sync_target(decay=0)
-  sync_net_weights(s, st);
+  const int na = (int)s->an.n, nc = (int)(2 * s->cn.n);
+  pdl_launch(k_pack, dim3((na + 255) / 256), dim3(256), 0, st, s->p_actor, na, dst_of(s, NETS_ACTOR));
+  pdl_launch(k_pack, dim3((nc + 255) / 256), dim3(256), 0, st, s->p_critic, nc, dst_of(s, NETS_CRITIC));
+  pdl_launch(k_pack, dim3((nc + 255) / 256), dim3(256), 0, st, s->p_target, nc, dst_of(s, NETS_TARGET));
+  s->launches += 3;
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 int b2q_sac_get_params(B2QSacHandle s, float* actor, float* critic, float* target, void* stream) {
@@ -708,26 +652,15 @@ int b2q_sac_phase(B2QSacHandle s, int phase, const float* obs, const float* act,
     if (critic_backward(s, st, src)) return -2;
   } else if (phase == 1 || phase == 3) {
     const float b1 = 0.9f, b2 = 0.999f;
-    auto dst_of = [&](const Net& nt, B2QMlpHandle mlp, int net, int bw /*index of the backward copies or -1*/, int a_off, int a_dim) {
-      PackDst d;
-      d.img = b2q_mlp_image(mlp, net);
-      d.W2T = bw >= 0 ? s->W2T[bw] : nullptr; d.W3T = bw >= 0 ? s->W3T[bw] : nullptr; d.W1A = (bw >= 0 && a_dim > 0) ? s->W1A[bw] : nullptr;
-      d.in_dim = nt.in_dim; d.od = nt.od; d.a_off = a_off; d.a_dim = a_dim; d.gradin = (bw >= 0 && a_dim > 0) ? 1 : 0;
-      d.oW1 = (unsigned)nt.oW1; d.ob1 = (unsigned)nt.ob1; d.oW2 = (unsigned)nt.oW2; d.ob2 = (unsigned)nt.ob2; d.oW3 = (unsigned)nt.oW3; d.ob3 = (unsigned)nt.ob3; d.n = (unsigned)nt.n;
-      return d;
-    };
     if (phase == 1) {                                 // critics: Adam + repack (forward images and backward copies) in one kernel
       int n = (int)(2 * cn.n);
-      PackDst2 dst; dst.d[0] = dst_of(cn, s->mlp_critic, 0, 1, D, A); dst.d[1] = dst_of(cn, s->mlp_critic, 1, 2, D, A);
-      pdl_launch(k_adam_pack, dim3((n + 255) / 256), dim3(256), 0, st, s->p_critic, s->g_critic, s->m_c, s->v_c, n, s->lr_c, b1, b2, 1e-8f, s->d_step, (int*)nullptr, dst);
+      pdl_launch(k_adam_pack, dim3((n + 255) / 256), dim3(256), 0, st, s->p_critic, s->g_critic, s->m_c, s->v_c, n, s->lr_c, b1, b2, 1e-8f, s->d_step, (int*)nullptr, dst_of(s, NETS_CRITIC));
       s->launches++;
     } else {                                          // actor Adam + repack on the caller's stream, Polyak + repack of the targets beside it
       int n = (int)an.n, nc = (int)(2 * cn.n);
       fork(s, st);
-      PackDst2 dt; dt.d[0] = dst_of(cn, s->mlp_target, 0, -1, 0, 0); dt.d[1] = dst_of(cn, s->mlp_target, 1, -1, 0, 0);
-      pdl_launch(k_polyak_pack, dim3((nc + 255) / 256), dim3(256), 0, s->side, s->p_target, s->p_critic, nc, s->tau, dt);
-      PackDst2 da; da.d[0] = dst_of(an, s->mlp_actor, 0, 0, 0, 0); da.d[1] = da.d[0];
-      pdl_launch(k_adam_pack, dim3((n + 255) / 256), dim3(256), 0, st, s->p_actor, s->g_actor, s->m_a, s->v_a, n, s->lr_a, b1, b2, 1e-8f, s->d_step, s->d_step + 1, da);
+      pdl_launch(k_polyak_pack, dim3((nc + 255) / 256), dim3(256), 0, s->side, s->p_target, s->p_critic, nc, s->tau, dst_of(s, NETS_TARGET));
+      pdl_launch(k_adam_pack, dim3((n + 255) / 256), dim3(256), 0, st, s->p_actor, s->g_actor, s->m_a, s->v_a, n, s->lr_a, b1, b2, 1e-8f, s->d_step, s->d_step + 1, dst_of(s, NETS_ACTOR));
       join(s, st);
       s->launches += 2;
     }
@@ -770,10 +703,10 @@ int b2q_sac_bc_learn(B2QSacHandle s, const float* obs, const float* ref_obs, int
                      const float* eps, float* losses_out, void* stream) {
   if (!s || !obs || !ref_obs || !expert_actor || !expert_critic || !eps) return -1;
   cudaStream_t st = (cudaStream_t)stream;
-  const int B = s->B, A = s->A, D = s->D, TB = 256, NB = (B + TB - 1) / TB;
-  const Net& an = s->an; const Net& cn = s->cn;
+  const int B = s->B, A = s->A, D = s->D, na = (int)s->an.n, nc = (int)(2 * s->cn.n);
+  const Net& an = s->an;
   cudaMemsetAsync(s->losses, 0, 4 * sizeof(float), st);
-  cudaMemsetAsync(s->g_actor, 0, (an.n + 2 * cn.n) * sizeof(float), st);
+  cudaMemsetAsync(s->g_actor, 0, (na + nc) * sizeof(float), st);
   s->actor_grad_dirty = true;
   // --- actor
   if (b2q_mlp_forward(expert_actor, ref_obs, ref_obs_dim, nullptr, B, B2Q_MLP_PREDICT, 0, nullptr, s->next_a /*ref action*/, nullptr, nullptr, st)) return -2;
@@ -781,19 +714,16 @@ int b2q_sac_bc_learn(B2QSacHandle s, const float* obs, const float* ref_obs, int
   if (b2q_mlp_forward_ex(s->mlp_actor, obs, D, nullptr, B, B2Q_MLP_RAW, 0, nullptr, s->raw_a, nullptr, nullptr, &sa, nullptr, nullptr, st)) return -2;
   pdl_launch(k_bc_dy, dim3(B / DY_ROWS), dim3(DY_ROWS * A), 0, st, s->raw_a, s->next_a, s->dy_rm, s->dy_bf, s->g_actor + an.ob3, s->losses + 1, B, A);
   if (actor_backward(s, st)) return -2;
-  pdl_launch(k_adam, dim3(((int)an.n + 255) / 256), dim3(256), 0, st, s->p_actor, s->g_actor, s->m_a, s->v_a, (int)an.n, s->lr_a, 0.9f, 0.999f, 1e-8f, s->d_step);
-  sync_net_weights(s, st, 1);
+  pdl_launch(k_adam_pack, dim3((na + 255) / 256), dim3(256), 0, st, s->p_actor, s->g_actor, s->m_a, s->v_a, na, s->lr_a, 0.9f, 0.999f, 1e-8f, s->d_step, (int*)nullptr, dst_of(s, NETS_ACTOR));
   // --- critic: a_now ~ pi_student(obs) (no grad); targets = expert Q(ref_obs, a_now)
   if (b2q_mlp_forward(s->mlp_actor, obs, D, nullptr, B, B2Q_MLP_SAMPLE, 0, eps, s->cur_a, s->cur_logp, nullptr, st)) return -2;
   if (b2q_mlp_forward(expert_critic, ref_obs, ref_obs_dim, s->cur_a, B, B2Q_MLP_RAW, 0, nullptr, s->qn, nullptr, nullptr, st)) return -2;
   B2QMlpSaves sv = {nullptr /*x row-major: no consumer*/, s->xc_t, s->hc1_rm, s->hc1_t, s->hc2_rm, s->hc2_t};
   if (b2q_mlp_forward_ex(s->mlp_critic, obs, D, s->cur_a, B, B2Q_MLP_RAW, 0, nullptr, s->q, nullptr, nullptr, &sv, nullptr, nullptr, st)) return -2;
-  pdl_launch(k_critic_dq, dim3(dim3(NB, 2)), dim3(TB), 0, st, s->q, s->qn, B, s->dq, s->losses + 0, B);
-  if (critic_backward(s, st)) return -2;
-  pdl_launch(k_adam, dim3(((int)(2 * cn.n) + 255) / 256), dim3(256), 0, st, s->p_critic, s->g_critic, s->m_c, s->v_c, (int)(2 * cn.n), s->lr_c, 0.9f, 0.999f, 1e-8f, s->d_step);
-  pdl_launch(k_step_inc, dim3(1), dim3(1), 0, st, s->d_step);        // both Adam kernels used step + 1; the step completes here
-  sync_net_weights(s, st, 2);
-  s->launches += 12;
+  if (critic_backward(s, st, DqSrc{DQ_TWIN, 0, s->q, nullptr, nullptr, s->qn, nullptr, 0.f, 0.f, s->losses + 0})) return -2;
+  // both Adam kernels used step + 1: the critics' closes the step
+  pdl_launch(k_adam_pack, dim3((nc + 255) / 256), dim3(256), 0, st, s->p_critic, s->g_critic, s->m_c, s->v_c, nc, s->lr_c, 0.9f, 0.999f, 1e-8f, s->d_step, s->d_step + 1, dst_of(s, NETS_CRITIC));
+  s->launches += 10;                                   // the two memsets and the eight kernels launched here (the backward helpers count their own)
   if (losses_out) cudaMemcpyAsync(losses_out, s->losses, 2 * sizeof(float), cudaMemcpyDeviceToDevice, st);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { s->err = cudaGetErrorString(e); return -2; }
