@@ -210,6 +210,9 @@ class PopulationEvaluator:
         return gather_fitness_and_length(self._fl, self.world, self.rank)
 
 
+DIVERGED_REWARD = -1e9      # the reward of an individual whose rollout went non-finite
+
+
 class DynamicsEvaluator:
     """Sim-to-real dynamics identification on the GPU (SURVEY §8f-4): the population of 48-vectors is mapped through
     param2dynamic_dict to per-env dynamics rows; every individual replays the recorded gait tables (ETG off, action =
@@ -240,7 +243,8 @@ class DynamicsEvaluator:
         self.reward = torch.zeros(self.n, dtype=dt, device=dev)
 
     def evaluate(self, solutions):
-        """solutions [pop,48] in [-1,1] (identical on every rank) -> reward [pop] = mean over the gait keys (identical on every rank)."""
+        """solutions [pop,48] in [-1,1] (identical on every rank) -> reward [pop] = mean over the gait keys (identical on every rank);
+        DIVERGED_REWARD for an individual whose rollout is non-finite."""
         import torch
         from .etg import dynamic_dict_to_row, param2dynamic_dict
         rows = np.array([dynamic_dict_to_row(param2dynamic_dict(np.asarray(s))) for s in np.asarray(solutions)[self.lo:self.hi]])
@@ -257,4 +261,7 @@ class DynamicsEvaluator:
                 assert rc == 0
         assert self.lib.b2q_dyn_finish(self.acc.data_ptr(), self.steps, self.reward.data_ptr(), self.n, es, stream) == 0
         local = self.reward.reshape(len(self.keys), pl).mean(0)        # (reward1 + reward2) / 2, :73
+        # a row whose robot diverges (light legs: the settle already ends in NaN) must rank last, not poison tell(): argsort puts NaN
+        # first in descending order, which would make the diverged individual the elite (same convention as train.py's ES phase)
+        local = torch.where(torch.isfinite(local), local, torch.full_like(local, DIVERGED_REWARD))
         return all_gather_concat(local.contiguous(), self.world, self.rank)

@@ -164,12 +164,30 @@ def _f32(x):
     return np.asarray(x, np.float64).astype(np.float32).astype(np.float64)
 
 
-def teacher_forced(eng, oracles, acts, flags, knee_rest=False):
+def ulps(x, n=4):
+    """x with every element moved by n float64 ulps (relative 2^-52 n), in a fixed alternating direction: the float64 counterpart of
+    _f32 for the sensitivity of a float64 engine."""
+    x = np.asarray(x, np.float64)
+    sign = np.where(np.arange(x.size) % 2 == 0, 1.0, -1.0).reshape(x.shape)
+    return x * (1.0 + sign * n * np.finfo(np.float64).eps)
+
+
+_HIST_AT, _HIST_LEN = O.Env.hist.offset, O.Env.hist_head.offset + C.sizeof(C.c_int) - O.Env.hist.offset   # hist, hist_len, hist_head
+
+
+def teacher_forced(eng, oracles, acts, flags, knee_rest=False, perturb=_f32):
     """Teacher-forced steps of an engine with n envs against n oracles.  `eng` has set_state([n,37]), get_state() -> [n,37] and
     step([n,A]) -> (obs, reward, done, info) as float64 numpy arrays.  Neither side resets: an env that falls goes on being compared
     (the knee contact rows only carry load once the robot is down).  Returns one record per (step, env):
-    (k, i, errors, oracle sensitivity, mismatch or None)."""
+    (k, i, errors, oracle sensitivity, mismatch or None).  The sensitivity is the oracle's response to `perturb` applied to its input
+    state and action: float32 rounding by default, `ulps` for a float64 engine.
+
+    Teacher forcing loads the state, not the observation history.  With a control latency longer than about one control step the
+    delayed observation of step k reads substeps of step k - 1 (and k - 2), which the engine computed itself.  So the sensitivity clone
+    carries its own history forward: from step 1 on it starts from the history its perturbed step left, and its response contains the
+    previous steps' rounding as the engine's does.  Before that, the history is the settled snapshot's (see full_range.warmup_steps)."""
     scratch = [O.OracleEnv(o.cfg, settle=False) for o in oracles]
+    hist = [None] * len(oracles)
     rec = []
     for k, a in enumerate(acts):
         eng.set_state(np.stack([o.get_state() for o in oracles]))
@@ -180,8 +198,12 @@ def teacher_forced(eng, oracles, acts, flags, knee_rest=False):
             oo, ro, do, io = o.step(a[i])
             so = o.get_state()
             c = pre[i]
-            c.set_state(_f32(c.get_state()))
-            sob, srw, _, sinf = c.step(_f32(a[i]))
+            if hist[i] is not None:
+                C.memmove(C.addressof(c.e) + _HIST_AT, hist[i], _HIST_LEN)
+            c.set_state(perturb(c.get_state()))
+            sob, srw, _, sinf = c.step(perturb(a[i]))
+            hist[i] = C.create_string_buffer(_HIST_LEN)
+            C.memmove(hist[i], C.addressof(c.e) + _HIST_AT, _HIST_LEN)
             rec.append((k, i, errors(ob[i], rw[i], inf[i], st[i], oo, ro, io, so, flags, knee_rest, o.cfg.reward_p),
                         errors(sob, srw, sinf, c.get_state(), oo, ro, io, so, flags, knee_rest, o.cfg.reward_p),
                         exact_mismatch(ob[i], dn[i], inf[i], oo, do, io, flags)))
