@@ -8,7 +8,8 @@
 #ifdef __cplusplus
 extern "C" {
 #endif
-/* writes n rows at ring positions (pos + i) % capacity. */
+/* writes n rows at ring positions (pos + i) % capacity.  valid_or_null is ignored: every row is written.  The masked append is
+ * b2q_rpm_append_masked_cursor below. */
 int b2q_rpm_append(float* s_obs, float* s_act, float* s_rew, float* s_next, float* s_term,
                    const float* obs, const float* act, const float* rew, const float* next_obs, const float* term, const uint8_t* valid_or_null,
                    int n, int obs_dim, int act_dim, int pos, int capacity, void* stream);
@@ -26,6 +27,14 @@ int b2q_rpm_append_cursor(float* s_obs, float* s_act, float* s_rew, float* s_nex
 int b2q_rpm_sample_cursor(const float* s_obs, const float* s_act, const float* s_rew, const float* s_next, const float* s_term,
                           float* obs, float* act, float* rew, float* next_obs, float* term, int batch, int obs_dim, int act_dim,
                           uint64_t seed, long long* state, void* stream);
+/* Masked append on the device cursor: writes exactly the rows with valid[i] != 0 (one byte per row), in ascending i, at
+ * (state[0] + rank_i) % capacity, rank_i = the number of valid rows before i; then advances position and fill level by the number of
+ * valid rows (the sample counter is unchanged).  That number stays on the device: no kernel argument depends on it and nothing
+ * synchronises, so a captured call replays correctly when the mask contents change.  1 <= n <= capacity; an all-zero mask changes
+ * nothing.  Two launches, deterministic. */
+int b2q_rpm_append_masked_cursor(float* s_obs, float* s_act, float* s_rew, float* s_next, float* s_term,
+                                 const float* obs, const float* act, const float* rew, const float* next_obs, const float* term,
+                                 const uint8_t* valid, int n, int obs_dim, int act_dim, int capacity, long long* state, void* stream);
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,64 @@ __global__ void rpm_sample_cursor_kernel(const float* s_obs, const float* s_act,
   if (t == 0) { rew[i] = s_rew[slot]; term[i] = s_term[slot]; }
 }
 __global__ void rpm_count_kernel(long long* state) { state[2] += 1; }
+
+// ---- masked append on the device cursor: row i goes to slot (state[0] + rank_i) % cap, rank_i = number of valid rows before i.  The call has
+//      no scratch memory, so each CTA recounts the mask before its tile (word loads); the grid is capped at MASK_MAX_CTAS so that this recount
+//      costs at most MASK_MAX_CTAS * n bytes of (L2-resident) reads.  The count of valid rows never leaves the device.
+constexpr int MASK_THREADS = 256, MASK_MAX_CTAS = 512;
+__device__ __forceinline__ int count_valid(const uint8_t* __restrict__ v, int end) {   // nonzero bytes of v[0, end) seen by this thread
+  int c = 0;
+  const int head = min(end, (int)((4 - ((uintptr_t)v & 3)) & 3));
+  for (int j = threadIdx.x; j < head; j += blockDim.x) c += v[j] != 0;
+  const uint32_t* w = (const uint32_t*)(v + head);
+  const int nw = (end - head) >> 2;
+  for (int j = threadIdx.x; j < nw; j += blockDim.x) c += __popc(__vcmpne4(__ldg(w + j), 0u)) >> 3;
+  for (int j = head + 4 * nw + threadIdx.x; j < end; j += blockDim.x) c += v[j] != 0;
+  return c;
+}
+__device__ __forceinline__ int block_sum(int x, int* red) {     // every thread gets the CTA's sum; red = 32 ints of shared memory
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = x;
+  __syncthreads();
+  int s = 0;
+  for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += red[w];
+  return s;
+}
+__global__ void __launch_bounds__(MASK_THREADS) rpm_append_masked_kernel(float* __restrict__ s_obs, float* __restrict__ s_act, float* __restrict__ s_rew,
+    float* __restrict__ s_next, float* __restrict__ s_term, const float* __restrict__ obs, const float* __restrict__ act, const float* __restrict__ rew,
+    const float* __restrict__ next_obs, const float* __restrict__ term, const uint8_t* __restrict__ valid, int n, int od, int ad, int cap, int tile,
+    const long long* __restrict__ state) {
+  __shared__ int red[32], rows[MASK_THREADS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = MASK_THREADS / 32;
+  const int lo = blockIdx.x * tile, hi = min(lo + tile, n);
+  long long base = state[0] + block_sum(count_valid(valid, lo), red);          // ring slot of this tile's first valid row (before the wrap)
+  for (int c0 = lo; c0 < hi; c0 += MASK_THREADS) {                                // chunks of 256 rows: ballot scan, compacted row list, warp per row
+    const int i = c0 + (int)threadIdx.x;
+    const bool f = i < hi && valid[i] != 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, f);
+    __syncthreads();                                                              // the previous chunk's copy has finished reading rows[]
+    if (lane == 0) red[warp] = __popc(bal);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int w = 0; w < nwarps; w++) { before += w < warp ? red[w] : 0; total += red[w]; }
+    if (f) rows[before + __popc(bal & ((1u << lane) - 1u))] = i;
+    __syncthreads();
+    for (int r = warp; r < total; r += nwarps) {
+      const size_t src = (size_t)rows[r], slot = (size_t)((base + r) % cap);
+      for (int k = lane; k < od; k += 32) { s_obs[slot * od + k] = obs[src * od + k]; s_next[slot * od + k] = next_obs[src * od + k]; }
+      for (int k = lane; k < ad; k += 32) s_act[slot * ad + k] = act[src * ad + k];
+      if (lane == 0) { s_rew[slot] = rew[src]; s_term[slot] = term[src]; }
+    }
+    base += total;
+  }
+}
+// one CTA, after the copy (stream order): advance position and fill level by the number of valid rows; the sample counter stays
+__global__ void __launch_bounds__(MASK_THREADS) rpm_advance_masked_kernel(long long* state, const uint8_t* __restrict__ valid, int n, int cap) {
+  __shared__ int red[32];
+  const int m = block_sum(count_valid(valid, n), red);
+  if (threadIdx.x == 0) { state[0] = (state[0] + m) % cap; state[1] = state[1] + m < cap ? state[1] + m : cap; }
+}
 }  // namespace
 
 extern "C" {
@@ -77,6 +135,15 @@ int b2q_rpm_sample_cursor(const float* s_obs, const float* s_act, const float* s
   if (!s_obs || !obs || !state || batch < 1) return -1;
   rpm_sample_cursor_kernel<<<batch, 64, 0, (cudaStream_t)stream>>>(s_obs, s_act, s_rew, s_next, s_term, obs, act, rew, next_obs, term, batch, od, ad, seed, state);
   rpm_count_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(state);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+int b2q_rpm_append_masked_cursor(float* s_obs, float* s_act, float* s_rew, float* s_next, float* s_term, const float* obs, const float* act, const float* rew,
+                                 const float* next_obs, const float* term, const uint8_t* valid, int n, int od, int ad, int cap, long long* state, void* stream) {
+  if (!s_obs || !s_act || !s_rew || !s_next || !s_term || !obs || !act || !rew || !next_obs || !term || !valid || !state || n < 1 || cap < n) return -1;
+  const int tile = 32 * ((n + 32 * MASK_MAX_CTAS - 1) / (32 * MASK_MAX_CTAS));
+  rpm_append_masked_kernel<<<(n + tile - 1) / tile, MASK_THREADS, 0, (cudaStream_t)stream>>>(s_obs, s_act, s_rew, s_next, s_term, obs, act, rew, next_obs, term,
+                                                                                            valid, n, od, ad, cap, tile, state);
+  rpm_advance_masked_kernel<<<1, MASK_THREADS, 0, (cudaStream_t)stream>>>(state, valid, n, cap);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 }

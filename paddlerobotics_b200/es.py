@@ -179,11 +179,20 @@ class PopulationEvaluator:
         self.policy, self.act_bound = policy, act_bound
         self.zero_act = torch.zeros(self.n, 12, dtype=dt, device=dev)
         self.es_launches = 0
+        self.rows = None
 
-    def evaluate(self, etg_w, etg_b, residual_noise=None):
+    def evaluate(self, etg_w, etg_b, residual_noise=None, replay=None, record=None):
         """etg_w [pop,3,20], etg_b [pop,3] for the WHOLE population (identical on every rank); returns fitness[pop]
-        (identical on every rank) and mean episode length[pop]."""
+        (identical on every rank) and mean episode length[pop].
+
+        replay: a ReplayMemory that receives the transitions whose reward enters the fitness (run_EStrain_episode with es_rpm,
+        train.py:240-241): on every step, the rows of the envs still in their first episode, of the FIRST rollout of each recorded
+        individual (the reference runs one episode per solution).  A row is (obs before the step, applied action / act_bound, reward,
+        next obs, 1 - done).  record: bool [pop] over the whole population, default all.  Needs an f32 evaluator.  Afterwards
+        `self.rows` (device int64 scalar) holds the number of rows this rank appended."""
         import torch
+        if replay is not None and self.env.dtype != torch.float32:
+            raise ValueError("evaluate(replay=...): the replay memory stores float32, so the evaluator must be built with precision='f32'")
         w = np.repeat(np.asarray(etg_w)[self.lo:self.hi], self.rollouts, axis=0)
         b = np.repeat(np.asarray(etg_b)[self.lo:self.hi], self.rollouts, axis=0)
         env = self.env
@@ -191,6 +200,14 @@ class PopulationEvaluator:
         self.alive.fill_(1); self.ret.zero_(); self.len.zero_()
         es = env.obs.element_size()
         stream = env._stream()
+        if replay is not None:
+            rec = np.ones(self.popsize, dtype=bool) if record is None else np.asarray(record, dtype=bool).reshape(self.popsize)
+            rec_local = torch.as_tensor(rec[self.lo:self.hi].astype(np.uint8), device=env.device)
+            keep = torch.zeros(self.pop_local, self.rollouts, dtype=torch.uint8, device=env.device)
+            keep[:, 0] = rec_local                                  # rollout 0 of each recorded individual
+            keep = keep.reshape(-1)
+            mask, prev_obs = torch.empty_like(keep), torch.empty_like(env.obs)
+            act_out, term, one = torch.empty_like(self.zero_act), torch.empty_like(self.ret), torch.ones_like(self.ret)
         for k in range(self.max_steps):
             if self.policy is not None:
                 act = self.policy(obs) * self.act_bound            # agent.predict(obs) * action_bound, train.py:226-228
@@ -198,7 +215,14 @@ class PopulationEvaluator:
                 act = self.zero_act
             if residual_noise is not None:
                 act = act + residual_noise[k]
+            if replay is not None:
+                prev_obs.copy_(obs)                                 # env.step overwrites env.obs in place
             obs, rew, done, _ = env.step(act, donef=(k + 1 > self.max_steps))
+            if replay is not None:                                  # the rows whose reward b2q_es_accumulate adds below
+                torch.mul(self.alive, keep, out=mask)
+                torch.div(act, self.act_bound, out=act_out)
+                torch.sub(one, done, out=term)                      # terminal = 1 - done, train.py:229-230
+                replay.append_masked(prev_obs, act_out, rew, obs, term, mask)
             rc = self.lib.b2q_es_accumulate(rew.data_ptr(), done.data_ptr(), self.alive.data_ptr(), self.ret.data_ptr(), self.len.data_ptr(),
                                             self.n, es, stream)
             assert rc == 0
@@ -207,6 +231,8 @@ class PopulationEvaluator:
                                      self.pop_local, self.rollouts, es, stream)
         assert rc == 0
         self.es_launches += 1
+        if replay is not None:
+            self.rows = (self.len.reshape(self.pop_local, self.rollouts)[:, 0].long() * rec_local).sum()
         return gather_fitness_and_length(self._fl, self.world, self.rank)
 
 

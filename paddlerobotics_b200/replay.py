@@ -21,17 +21,61 @@ class ReplayMemory:
         self.action, self.reward, self.terminal = z(self.max_size, act_dim), z(self.max_size), z(self.max_size)
         self._curr_size, self._curr_pos, self._samples = 0, 0, 0
         self.cursor = torch.zeros(3, dtype=torch.int64, device=self.device) if device_cursor else None   # {position, fill level, samples}
+        # append_masked: how many rows it wrote is known only on the device, so it runs on a device cursor (self.cursor, or in host-cursor
+        # mode this one, loaded from the host mirrors) and leaves the mirrors stale until sync_host() reads that cursor back
+        self._masked_cursor = None
+        self._stale = False
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
+    def sync_host(self):
+        """Brings the host mirrors (size(), the host-cursor position) up to date after masked appends with one device-to-host read of
+        the cursor.  In device-cursor mode it always reads (call it after replaying a CUDA graph that contains a masked append); in
+        host-cursor mode only when a masked append ran since the last read.  size(), append, advance and sample_batch catch up by
+        themselves after eager masked appends."""
+        if self.cursor is not None:
+            self._stale = True
+        self._refresh()
+
+    def _refresh(self):
+        if self._stale:
+            self._curr_pos, self._curr_size = (int(x) for x in (self.cursor if self.cursor is not None else self._masked_cursor)[:2].tolist())
+            self._stale = False
+
     def size(self):
+        self._refresh()
         return self._curr_size
 
     def __len__(self):
-        return self._curr_size
+        return self.size()
+
+    def append_masked(self, obs, act, reward, next_obs, terminal, mask):
+        """Appends the rows i with mask[i] != 0, in row order (one row per env whose transition is kept, e.g. the envs still in their
+        first episode).  The number of rows written never reaches the host (b2q_rpm_append_masked_cursor): no sync, and in device-cursor
+        mode the call can be captured in a CUDA graph and replayed with new mask contents."""
+        t = lambda x: torch.as_tensor(x, dtype=torch.float32, device=self.device).contiguous()
+        obs, act, reward, next_obs, terminal = t(obs).reshape(-1, self.obs_dim), t(act).reshape(-1, self.act_dim), t(reward).reshape(-1), t(next_obs).reshape(-1, self.obs_dim), t(terminal).reshape(-1)
+        mask = torch.as_tensor(mask, device=self.device).to(torch.uint8).contiguous().reshape(-1)
+        n = obs.shape[0]
+        if not (act.shape[0] == reward.shape[0] == next_obs.shape[0] == terminal.shape[0] == mask.shape[0] == n):
+            raise ValueError("append_masked: obs, act, reward, next_obs, terminal and mask must have the same number of rows")
+        cursor = self.cursor
+        if cursor is None:
+            if self._masked_cursor is None:
+                self._masked_cursor = torch.zeros(3, dtype=torch.int64, device=self.device)
+            cursor = self._masked_cursor
+            if not self._stale:                  # the host mirrors hold the position: load them (fills, no sync)
+                cursor[0], cursor[1], cursor[2] = self._curr_pos, self._curr_size, self._samples
+        rc = self.lib.b2q_rpm_append_masked_cursor(self.obs.data_ptr(), self.action.data_ptr(), self.reward.data_ptr(), self.next_obs.data_ptr(), self.terminal.data_ptr(),
+                                                   obs.data_ptr(), act.data_ptr(), reward.data_ptr(), next_obs.data_ptr(), terminal.data_ptr(), mask.data_ptr(),
+                                                   n, self.obs_dim, self.act_dim, self.max_size, cursor.data_ptr(), self._stream())
+        assert rc == 0, rc
+        self._keep_masked = (obs, act, reward, next_obs, terminal, mask)      # inputs of a captured launch must outlive the capture
+        self._stale = True
 
     def append(self, obs, act, reward, next_obs, terminal):
+        self._refresh()
         t = lambda x: torch.as_tensor(x, dtype=torch.float32, device=self.device).contiguous()
         obs, act, reward, next_obs, terminal = t(obs).reshape(-1, self.obs_dim), t(act).reshape(-1, self.act_dim), t(reward).reshape(-1), t(next_obs).reshape(-1, self.obs_dim), t(terminal).reshape(-1)
         n = obs.shape[0]
@@ -53,6 +97,7 @@ class ReplayMemory:
 
     def advance(self, n, samples=1):
         """Host-side mirrors only: a captured iteration (device cursor) was replayed — n rows appended, `samples` minibatches drawn."""
+        self._refresh()
         self._curr_pos = (self._curr_pos + n) % self.max_size
         self._curr_size = min(self._curr_size + n, self.max_size)
         self._samples += samples
@@ -60,6 +105,7 @@ class ReplayMemory:
     def sample_batch(self, batch_size, seed=None, out=None):
         """Uniform sample (replay_memory.py sample_batch).  out = (obs, act, rew, next_obs, term) float32 device tensors to gather into
         (e.g. SACLearner.static_batch(): the learner's CUDA-graph inputs are then filled in place, with no copy in between)."""
+        self._refresh()
         self._samples += 1
         if out is not None:
             obs, act, rew, nobs, term = out

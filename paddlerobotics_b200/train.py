@@ -40,6 +40,8 @@ def main(argv=None):
     p.add_argument("--es_rollouts", type=int, default=4)
     p.add_argument("--es_every_steps", type=int, default=200000)       # ES_EVERY_STEPS = 5e4 per env in the reference
     p.add_argument("--es_train_steps", type=int, default=3)            # ES_TRAIN_STEPS = 10
+    p.add_argument("--es_rpm", type=int, default=0, help="1: the ES phase also feeds SAC: the incumbent's episode and the first rollout of every "
+                   "individual are appended to the replay memory (run_EStrain_episode, train.py:240-241; the reference's default is 1)")
     p.add_argument("--sigma", type=float, default=0.02)
     p.add_argument("--sigma_decay", type=float, default=0.99)
     p.add_argument("--seed", type=int, default=0)
@@ -173,20 +175,32 @@ def main(argv=None):
         if evaluator is not None and total - last_es >= args.es_every_steps and rpm.size() >= args.warmup_steps:
             last_es = total
             # the incumbent ETG seeds best_reward (train.py:395-396): a sampled individual replaces it only if it is actually better
-            inc_fit, _ = evaluator.evaluate(np.repeat(np.asarray(w)[None], args.popsize, 0), np.repeat(np.asarray(b)[None], args.popsize, 0))
+            es_replay = rpm if args.es_rpm else None
+            # popsize copies of ONE gait: only one episode goes to the replay (train.py:395)
+            inc_fit, _ = evaluator.evaluate(np.repeat(np.asarray(w)[None], args.popsize, 0), np.repeat(np.asarray(b)[None], args.popsize, 0),
+                                            replay=es_replay, record=np.arange(args.popsize) == 0)
+            es_rows = [int(evaluator.rows)] if args.es_rpm else []
             inc = inc_fit.double().cpu().numpy()
             best_fit = float(np.nanmean(inc)) if np.isfinite(inc).any() else -np.inf
             best_param = ETG_best_param.copy()
             for gen in range(args.es_train_steps):                                     # train.py:397-418
                 sol = solver.ask()
                 ws, bs = solutions_to_etg_device(sol, prior_points, w0, b0, ETG_T=args.ETG_T)
-                fit, mlen = evaluator.evaluate(ws.cpu().numpy(), bs.cpu().numpy())
+                fit, mlen = evaluator.evaluate(ws.cpu().numpy(), bs.cpu().numpy(), replay=es_replay)
                 fit_np = fit.double().cpu().numpy()
                 fit_np = np.where(np.isfinite(fit_np), fit_np, -1e9)                    # a diverged rollout must lose, not poison tell()
                 solver.tell(fit_np)
                 if fit_np.max() > best_fit:
                     best_fit, best_param = float(fit_np.max()), np.asarray(sol[int(fit_np.argmax())]).copy()
-                print(json.dumps({"ES_gen": gen, "fitness_max": float(fit_np.max()), "fitness_mean": float(fit_np.mean()), "mean_len": float(mlen.mean())}), flush=True)
+                rec = {"ES_gen": gen, "fitness_max": float(fit_np.max()), "fitness_mean": float(fit_np.mean()), "mean_len": float(mlen.mean())}
+                if args.es_rpm:
+                    es_rows.append(int(evaluator.rows))
+                    rec["rpm_rows"] = es_rows[-1]
+                print(json.dumps(rec), flush=True)
+            if args.es_rpm:
+                # the masked appends advanced the ring's device cursor; one read brings the host mirrors level before the loop uses them
+                rpm.sync_host()
+                print(json.dumps({"ES_rpm_rows": sum(es_rows), "env_steps": total, "rpm_size": rpm.size()}), flush=True)
             ETG_best_param = best_param
             pts = prior_points + ETG_best_param.reshape(-1, 2)                          # train.py:433-437
             w, b, _ = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, w0=w0, b0=b0, points=pts)

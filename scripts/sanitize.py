@@ -75,5 +75,13 @@ for i in range(2):
 wide.forward(torch.randn(129, 52, device="cuda"), in2=torch.randn(129, 12, device="cuda"), mode=1, seed=5)
 ev = PopulationEvaluator(4, 2, max_steps=5)
 ev.evaluate(np.repeat(w[None], 4, 0), np.repeat(b[None], 4, 0))
+# masked appends on the device cursor: a partial mask whose rows cross the ring's wrap (100 rows, 60 valid, from position 4050 of 4096),
+# then the ES evaluator feeding a host-cursor ring
+mrpm = ReplayMemory(4096, 49, 12, device_cursor=True)
+mrpm.cursor[0] = 4050
+mrpm.append_masked(torch.randn(100, 49, device="cuda"), torch.rand(100, 12, device="cuda"), torch.randn(100, device="cuda"), torch.randn(100, 49, device="cuda"),
+                   torch.ones(100, device="cuda"), torch.arange(100, device="cuda") % 5 < 3)
+mrpm.sync_host()
+ev.evaluate(np.repeat(w[None], 4, 0), np.repeat(b[None], 4, 0), replay=rpm)
 torch.cuda.synchronize()
 print("sanitizer script done")
