@@ -23,7 +23,9 @@ int b2q_etg_fit(const double* obs6x20, const double* prior_points, const double*
                 double precision, double* w_out, double* b_out, int pop, void* stream);
 /* Dynamics identification (SURVEY §8f-4): loss_func of model/Dynamic_parallel_model.py:29-41 accumulated on the device.
  * info [n,56] is the step kernel's info output; mean15/std15 = recorded {motor12, drpy3} statistics of THIS control step;
- * acc [n,15] running sums (zero it before an episode); reward[n] = 30 - (max_j mean_t motor_j + max_k mean_t drpy_k)/2. */
+ * acc [n,15] running sums (zero it before an episode); reward[n] = 30 - (max_j mean_t motor_j + max_k mean_t drpy_k)/2.
+ * The maxima propagate NaN as the reference's np.max does: a NaN in any one of an env's 15 columns makes its reward NaN, and +inf in
+ * one (with no NaN) makes it -inf, so a caller that maps non-finite rewards to a floor (es.DynamicsEvaluator) sees every such env. */
 int b2q_dyn_accumulate(const void* info, const void* mean15, const void* std15, void* acc, int n, int elem_size, void* stream);
 int b2q_dyn_finish(const void* acc, int steps, void* reward, int n, int elem_size, void* stream);
 #ifdef __cplusplus

@@ -122,13 +122,16 @@ __global__ void dyn_accum_kernel(const T* __restrict__ info /*[N][56]*/, const T
   T d = x - mean15[c], s = std15[c];
   acc[i] += d * d / (s * s);
 }
+// max that propagates NaN like the reference's np.max (fmax drops it: a NaN column would leave a finite reward from the other 14)
+template <typename T>
+__device__ __forceinline__ T max_nan(T a, T b) { return (a != a || a > b) ? a : b; }
 template <typename T>
 __global__ void dyn_finish_kernel(const T* __restrict__ acc, int steps, T* __restrict__ reward, int n) {
   int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n) return;
   T lm = acc[(size_t)e * 15], ld = acc[(size_t)e * 15 + 12];
-  for (int c = 1; c < 12; c++) lm = fmax(lm, acc[(size_t)e * 15 + c]);
-  for (int c = 13; c < 15; c++) ld = fmax(ld, acc[(size_t)e * 15 + c]);
+  for (int c = 1; c < 12; c++) lm = max_nan(lm, acc[(size_t)e * 15 + c]);
+  for (int c = 13; c < 15; c++) ld = max_nan(ld, acc[(size_t)e * 15 + c]);
   reward[e] = T(30) - (lm / T(steps) + ld / T(steps)) / T(2);
 }
 }  // namespace

@@ -83,5 +83,19 @@ mrpm.append_masked(torch.randn(100, 49, device="cuda"), torch.rand(100, 12, devi
                    torch.ones(100, device="cuda"), torch.arange(100, device="cuda") % 5 < 3)
 mrpm.sync_host()
 ev.evaluate(np.repeat(w[None], 4, 0), np.repeat(b[None], 4, 0), replay=rpm)
+# masked append with several 256-row chunks per CTA (n = 131073: tiles of 288 rows), cap == n, then a mask 3 bytes past a word boundary
+# (count_valid's byte-wise head), both through ReplayMemory.append_masked
+n = 131073
+big = ReplayMemory(n, 49, 12, device_cursor=True)
+big.cursor[0] = 7
+big.append_masked(torch.randn(n, 49, device="cuda"), torch.rand(n, 12, device="cuda"), torch.randn(n, device="cuda"), torch.randn(n, 49, device="cuda"),
+                  torch.ones(n, device="cuda"), torch.rand(n, device="cuda") < 0.5)
+mbuf = torch.ones(1003, dtype=torch.uint8, device="cuda")
+big.append_masked(torch.randn(1000, 49, device="cuda"), torch.rand(1000, 12, device="cuda"), torch.randn(1000, device="cuda"), torch.randn(1000, 49, device="cuda"),
+                  torch.ones(1000, device="cuda"), mbuf[3:])
+big.sync_host()
+# ES fitness with 33 rollouts per individual: lane 0 runs the strided loop twice
+evr = PopulationEvaluator(3, 33, max_steps=2)
+evr.evaluate(np.repeat(w[None], 3, 0), np.repeat(b[None], 3, 0))
 torch.cuda.synchronize()
 print("sanitizer script done")

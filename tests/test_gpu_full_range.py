@@ -203,3 +203,44 @@ def test_dynamics_identification_ranks_diverged_individuals_last(torch_cuda, gol
                         motor.append(info[42:54]); drpy.append(info[39:42])
                     ref[i] += (30 - loss_np(np.array(drpy), np.array(motor), md, k)) / 2.0
             assert np.abs(rew[~diverged] - ref[~diverged]).max() < 1e-6, (rew, ref)
+
+
+def test_dynamics_identification_ranks_a_nan_loss_column_diverged(torch_cuda):
+    """An individual whose rollout is finite but whose accumulated loss has NaN in ONE of its 15 columns (one joint angle, or one body
+    rate) is non-finite only through b2q_dyn_finish's maxima: it must score es.DIVERGED_REWARD.  With a NaN-dropping max (fmax) its
+    reward came out finite from the other 14 columns, so it could become the elite.  The untouched individuals keep their rewards."""
+    from paddlerobotics_b200.es import DIVERGED_REWARD, DynamicsEvaluator
+    T = 5
+    tab = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gait_action_list_CPG_stairstair7_12_3.npy")) + np.array([0, 0.9, -1.8] * 4)
+    gait = {"exp": tab[:T], "ori": tab[100:100 + T]}
+    rng = np.random.default_rng(1)
+    md = {}
+    for k in ("exp", "ori"):
+        md[k + "_motor_mean"] = gait[k] + rng.normal(0, 0.02, (T, 12)); md[k + "_motor_std"] = rng.uniform(0.05, 0.1, (T, 12))
+        md[k + "_drpy_mean"] = rng.normal(0, 0.2, (T, 3)); md[k + "_drpy_std"] = rng.uniform(0.3, 0.6, (T, 3))
+    sols = rng.uniform(-0.2, 0.2, (4, 48))
+
+    class Poisoned:
+        """The library, except that dyn_finish first sets acc[env, col] = value for each entry of `poison`."""
+
+        def __init__(self, lib, acc, poison):
+            self.lib, self.acc, self.poison = lib, acc, poison
+
+        def __getattr__(self, name):
+            return getattr(self.lib, name)
+
+        def b2q_dyn_finish(self, *args):
+            for env, col, value in self.poison:
+                self.acc[env, col] = value
+            return self.lib.b2q_dyn_finish(*args)
+
+    for precision in ("f32", "f64"):
+        ev = DynamicsEvaluator(4, gait, md, steps=T, precision=precision)
+        clean = ev.evaluate(sols).double().cpu().numpy()
+        assert np.isfinite(clean).all() and (clean > DIVERGED_REWARD).all(), clean
+        # env = key * pop + individual: individual 1's joint-angle column 4 on the "exp" gait, individual 2's body-rate column 13 on "ori"
+        ev.lib = Poisoned(ev.lib, ev.acc, [(1, 4, float("nan")), (4 + 2, 13, float("nan"))])
+        rew = ev.evaluate(sols).double().cpu().numpy()
+        ev.env.close()
+        assert rew[1] == DIVERGED_REWARD and rew[2] == DIVERGED_REWARD, (precision, rew)
+        assert rew[0] == clean[0] and rew[3] == clean[3], (precision, rew, clean)
