@@ -66,6 +66,8 @@ SYMBOLS = {
     "b2q_rpm_append_cursor": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "b2q_rpm_sample_cursor": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, C.c_uint64, _vp, _vp]),
     "b2q_rpm_append_masked_cursor": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u8p, _i, _i, _i, _i, _vp, _vp]),
+    # camera images — include/b2q_render.h
+    "b2q_render": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
 }
 
 

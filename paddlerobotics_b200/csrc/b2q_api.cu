@@ -10,6 +10,8 @@
 #include <new>
 #include <string>
 #include "b2q_host_common.h"
+#include "b2q_render_internal.h"
+#include "../../include/b2q_render.h"
 
 using namespace b2q;
 
@@ -191,6 +193,8 @@ struct EnvBase {
   virtual int get_state(void* out, cudaStream_t s) = 0;
   virtual int set_state(const void* in, cudaStream_t s) = 0;
   virtual int get_step_count(int32_t* out, cudaStream_t s) = 0;
+  virtual int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
+                     int32_t* seg, cudaStream_t s) = 0;
 };
 
 #define CK(call)                                                                      \
@@ -211,6 +215,7 @@ struct EnvT : EnvBase {
   T* d_hf = nullptr;
   void* d_pool = nullptr;
   int tpb = 32;
+  float hf_lo = 0.0f, hf_hi = 0.0f;
 
   ~EnvT() override {
     cudaSetDevice(cfg.device);
@@ -234,6 +239,8 @@ struct EnvT : EnvBase {
       T* tmp = (T*)malloc(n * sizeof(T));
       if (!tmp) { err = "host alloc failed"; return B2Q_ENOMEM; }
       for (size_t i = 0; i < n; i++) tmp[i] = (T)c.hf_host[i];
+      hf_lo = hf_hi = (float)tmp[0];   // height range of the field: the camera rays are clipped to it (b2q_render)
+      for (size_t i = 0; i < n; i++) { hf_lo = std::fmin(hf_lo, (float)tmp[i]); hf_hi = std::fmax(hf_hi, (float)tmp[i]); }
       cudaError_t e1 = cudaMalloc(&d_hf, n * sizeof(T));
       if (e1 == cudaSuccess) e1 = cudaMemcpy(d_hf, tmp, n * sizeof(T), cudaMemcpyHostToDevice);
       free(tmp);
@@ -403,6 +410,23 @@ struct EnvT : EnvBase {
     CK(cudaMemcpyAsync(out, B.step_count, sizeof(int) * B.N, cudaMemcpyDeviceToDevice, s));
     return B2Q_OK;
   }
+  int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
+             int32_t* seg, cudaStream_t s) override {
+    if (!state || !env_ids || !view || !proj) { err = "b2q_render: null state, env_ids, view or proj"; return B2Q_EINVAL; }
+    if (V < 1 || V > 65535) { err = "b2q_render: V must be in [1, 65535]"; return B2Q_EINVAL; }
+    if (W < 1 || H < 1 || W > 16384 || H > 16384) { err = "b2q_render: width and height must be in [1, 16384]"; return B2Q_EINVAL; }
+    if ((size_t)rgba & 3) { err = "b2q_render: rgba must be 4-byte aligned"; return B2Q_EINVAL; }
+    CK(cudaSetDevice(cfg.device));
+    RenderArgs<T> a;
+    build_model_host(a.md, cfg.foot_radius, cfg.etg_T, cfg.etg_amp, cfg.etg_phase0, cfg.etg_phase1, cfg.etg_foot_y_inset);
+    a.tr.type = kc.terrain; a.tr.nx = kc.hf_nx; a.tr.ny = kc.hf_ny;
+    a.tr.x0 = (float)cfg.hf_x0; a.tr.y0 = (float)cfg.hf_y0; a.tr.icell = (float)kc.hf_icell; a.tr.lo = hf_lo; a.tr.hi = hf_hi;
+    a.hf = d_hf; a.state = (const T*)state; a.N = B.N; a.env_ids = env_ids; a.view = view; a.proj = proj;
+    a.W = W; a.H = H; a.rgba = rgba; a.depth = depth; a.seg = seg;
+    CK(render_launch<T>(a, V, s));
+    launches++;
+    return B2Q_OK;
+  }
 };
 
 }  // namespace
@@ -457,5 +481,9 @@ int b2q_get_state(B2QHandle h, void* out, void* s) { return h ? h->impl->get_sta
 int b2q_set_state(B2QHandle h, const void* in, void* s) { return h ? h->impl->set_state(in, (cudaStream_t)s) : B2Q_EINVAL; }
 int b2q_get_step_count(B2QHandle h, int32_t* out, void* s) { return h ? h->impl->get_step_count(out, (cudaStream_t)s) : B2Q_EINVAL; }
 int64_t b2q_launch_count(B2QHandle h) { return h ? h->impl->launches : 0; }
+int b2q_render(B2QHandle h, const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int width, int height, uint8_t* rgba,
+               float* depth, int32_t* seg, void* stream) {
+  return h ? h->impl->render(state, env_ids, V, view, proj, width, height, rgba, depth, seg, (cudaStream_t)stream) : B2Q_EINVAL;
+}
 
 }  // extern "C"

@@ -125,6 +125,49 @@ class VecQuadrupedalEnv:
     def launch_count(self):
         return int(self.lib.b2q_launch_count(self.h))
 
+    def get_camera_image(self, width=640, height=480, env_ids=None, view=None, proj=None):
+        """Ray-cast camera images of the current state (b2q_render, include/b2q_render.h): view v shows env env_ids[v] (default
+        every env).  view / proj: [16] (one matrix for every view) or [V,16] column-major pybullet matrices; None = the follow
+        camera of each env (render.follow_camera).  Returns device tensors (rgba [V,H,W,4] uint8, depth [V,H,W] float32 OpenGL
+        depth-buffer values, seg [V,H,W] int32), which the next call with the same sizes overwrites: the buffers are reused, so the
+        call can be captured in a CUDA graph (pass env_ids / view / proj as device tensors or None there)."""
+        from . import render
+        dev, W, H = self.device, int(width), int(height)
+        if env_ids is None:
+            if getattr(self, "_r_all", None) is None:
+                self._r_all = torch.arange(self.num_envs, dtype=torch.int32, device=dev)
+            ids = self._r_all
+        else:
+            ids = torch.as_tensor(env_ids, device=dev).to(torch.int32).reshape(-1).contiguous()
+        V = int(ids.shape[0])
+        key = (V, H, W)
+        if getattr(self, "_r_key", None) != key:
+            self._r_key = key
+            self._r_rgba = torch.empty(V, H, W, 4, dtype=torch.uint8, device=dev)
+            self._r_depth = torch.empty(V, H, W, dtype=torch.float32, device=dev)
+            self._r_seg = torch.empty(V, H, W, dtype=torch.int32, device=dev)
+            self._r_view = torch.empty(V, 16, dtype=torch.float32, device=dev)
+            self._r_proj = torch.empty(V, 16, dtype=torch.float32, device=dev)
+            self._r_proj_hw = None
+        if getattr(self, "_r_state", None) is None:
+            self._r_state = torch.empty(self.num_envs, STATE_DIM, device=dev, dtype=self.dtype)
+        _check(self.lib, self.h, self.lib.b2q_get_state(self.h, self._r_state.data_ptr(), self._stream()), "b2q_get_state")
+        if view is None:
+            render.follow_view_matrices(self._r_state.index_select(0, ids.clamp(0, self.num_envs - 1).long())[:, :3], self._r_view)
+        else:
+            self._r_view.copy_(torch.as_tensor(view, dtype=torch.float32, device=dev).reshape(-1, 16).expand(V, 16))
+        if proj is None:
+            if self._r_proj_hw != (H, W):     # the default projection depends on the aspect only: uploaded once per size
+                self._r_proj.copy_(torch.tensor(render.follow_camera((0, 0, 0), W, H)[1], dtype=torch.float32, device=dev).expand(V, 16))
+                self._r_proj_hw = (H, W)
+        else:
+            self._r_proj.copy_(torch.as_tensor(proj, dtype=torch.float32, device=dev).reshape(-1, 16).expand(V, 16))
+            self._r_proj_hw = None
+        rc = self.lib.b2q_render(self.h, self._r_state.data_ptr(), ids.data_ptr(), V, self._r_view.data_ptr(), self._r_proj.data_ptr(), W, H,
+                                   self._r_rgba.data_ptr(), self._r_depth.data_ptr(), self._r_seg.data_ptr(), self._stream())
+        _check(self.lib, self.h, rc, "b2q_render")
+        return self._r_rgba, self._r_depth, self._r_seg
+
     # ------------------------------------------------------------------ host API (numpy in / numpy out)
     def _host_bufs(self):
         if self._h_act is None:
@@ -305,6 +348,12 @@ class QuadrupedalEnv:
         # one C call + one stream sync: actions in, obs / reward / done / info out through pinned host buffers
         obs, rew, done, info = self.vec.step_host(np.asarray(action).reshape(1, self.vec.action_dim), donef, info=True)
         return obs[0].astype(np.float64), float(rew[0]), bool(done[0]), info_dict(info[0])
+
+    def get_camera_image(self, width=640, height=480, viewMatrix=None, projectionMatrix=None):
+        """pybullet.getCameraImage(width, height, viewMatrix, projectionMatrix) -> (width, height, rgba [H,W,4] uint8,
+        depth [H,W] float32, seg [H,W] int32) as numpy arrays (train.py:197).  No matrices = the follow camera."""
+        rgba, depth, seg = self.vec.get_camera_image(width, height, view=viewMatrix, proj=projectionMatrix)
+        return int(width), int(height), rgba[0].cpu().numpy(), depth[0].cpu().numpy(), seg[0].cpu().numpy()
 
     def close(self):
         self.vec.close()

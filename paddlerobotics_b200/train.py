@@ -57,6 +57,11 @@ def main(argv=None):
     p.add_argument("--suffix", type=str, default="exp0")
     p.add_argument("--eval_every_steps", type=int, default=0, help="checkpoint cadence in env steps; 0 = EVAL_EVERY_STEPS (1e4) per env")
     p.add_argument("--load", type=str, default="", help="itr_*.pt to restore the agent from (and the .npz next to it for w, b, param)")
+    p.add_argument("--eval", type=int, default=0, help="1: evaluate the --load checkpoint instead of training (run_evaluate_episodes, train.py:182-211,438-449)")
+    p.add_argument("--eval_envs", type=int, default=1, help="envs of the --eval episode (one episode each, no auto-reset)")
+    p.add_argument("--render_dir", type=str, default="", help="--eval: write env 0's camera image of every step to DIR/img{step}.png (train.py:196-199); empty = no frames")
+    p.add_argument("--render_width", type=int, default=640)
+    p.add_argument("--render_height", type=int, default=480)
     args = p.parse_args(argv)
     torch.manual_seed(args.seed); np.random.seed(args.seed)
     n = args.num_envs
@@ -68,6 +73,10 @@ def main(argv=None):
     env_cfg = dict(w_torso=args.torso, w_feet=args.feet, w_up=args.up, w_tau=args.tau, w_badfoot=args.badfoot, w_footcontact=args.footcontact,
                    heightfield=make_terrain(args.task_mode, step_y=args.step_y), stuck_termination=1, body_collisions=1,
                    etg_foot_y_inset=args.step_y if args.task_mode == "balancebeam" else 0.0)
+    if args.eval:
+        if not args.load:
+            p.error("--eval 1 evaluates a checkpoint: it needs --load itr_*.pt")
+        return evaluate(args, env_cfg)
     env = VecQuadrupedalEnv(n, auto_reset=True, max_episode_steps=args.e_step, **env_cfg)
     agent = MujocoAgent(49, 12, seed=args.seed)
     ETG_best_param = np.zeros(12)                                                                                                 # ES_solver.get_best_param(), train.py:348
@@ -209,6 +218,54 @@ def main(argv=None):
     torch.cuda.synchronize()
     learner.pull()
     return log
+
+
+EVAL_MAX_STEP = 600                                                         # run_evaluate_episodes(agent, env, 600, ...), train.py:445
+EVAL_TERMS = ("torso", "feet", "up", "tau", "badfoot", "footcontact")       # the info terms summed per episode, train.py:202-207
+
+
+def evaluate(args, env_cfg):
+    """--eval 1: one deterministic episode per env of the restored agent and ETG (w, b) on the training env's config, at most
+    EVAL_MAX_STEP + 1 control steps (the reference's loop breaks after step 601).  Each env's return, length and per-term sums are
+    frozen at its first done by the ES evaluator's accumulator (b2q_es_accumulate).  Prints and returns one JSON record."""
+    from . import _lib
+    from ._config import INFO
+    from .render import write_png
+    agent = MujocoAgent(49, 12, seed=args.seed)
+    agent.restore(args.load)
+    z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
+    w, b = z["w"], z["b"]
+    n = args.eval_envs
+    env = VecQuadrupedalEnv(n, auto_reset=False, **env_cfg)
+    lib, dev, es, stream = _lib.load(), env.device, env.obs.element_size(), env._stream()
+    if args.render_dir:
+        os.makedirs(args.render_dir, exist_ok=True)
+    nt = len(EVAL_TERMS)
+    cols = torch.tensor([INFO[k] for k in EVAL_TERMS], device=dev)
+    alive = torch.ones(n, dtype=torch.uint8, device=dev)
+    ret, length = torch.zeros(n, dtype=env.dtype, device=dev), torch.zeros(n, dtype=torch.int32, device=dev)
+    # every term gets its own copy of `alive` per step (the accumulator clears it at done), so all sums freeze at the same step
+    t_alive, t_sum, t_len = torch.empty(nt, n, dtype=torch.uint8, device=dev), torch.zeros(nt, n, dtype=env.dtype, device=dev), torch.zeros(nt, n, dtype=torch.int32, device=dev)
+    t_val = torch.empty(nt, n, dtype=env.dtype, device=dev)
+    obs = env.reset(w, b)
+    for steps in range(1, EVAL_MAX_STEP + 2):
+        act = agent.predict_batch(obs)                                                                        # agent.predict(obs), train.py:193
+        obs, rew, done, info = env.step(act * args.act_bound, donef=steps > EVAL_MAX_STEP)
+        if args.render_dir:
+            rgba = env.get_camera_image(args.render_width, args.render_height, env_ids=[0])[0]
+            write_png(os.path.join(args.render_dir, "img%d.png" % steps), rgba[0].cpu().numpy())
+        t_val.copy_(info.index_select(1, cols).T)
+        t_alive.copy_(alive.expand(nt, n))
+        for j in range(nt):
+            assert lib.b2q_es_accumulate(t_val[j].data_ptr(), done.data_ptr(), t_alive[j].data_ptr(), t_sum[j].data_ptr(), t_len[j].data_ptr(), n, es, stream) == 0
+        assert lib.b2q_es_accumulate(rew.data_ptr(), done.data_ptr(), alive.data_ptr(), ret.data_ptr(), length.data_ptr(), n, es, stream) == 0
+        if not bool(alive.any()):
+            break
+    rec = {"eval_envs": n, "mean_return": float(ret.double().mean()), "mean_length": float(length.double().mean()),
+           "terms": {k: float(t_sum[j].double().mean()) for j, k in enumerate(EVAL_TERMS)}}
+    print(json.dumps(rec), flush=True)
+    env.close()
+    return rec
 
 
 if __name__ == "__main__":
