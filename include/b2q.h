@@ -145,6 +145,10 @@ int b2q_set_state(B2QHandle h, const void* state_in /*[N,37]*/, void* stream);
 int b2q_get_step_count(B2QHandle h, int32_t* out /*[N] device*/, void* stream);
 /* number of kernels this handle has launched so far (bench.py's gpu_launches) */
 int64_t b2q_launch_count(B2QHandle h);
+/* changes cfg.max_episode_steps for every following step (BCtrain.py:313-314 lengthens the episodes during a run); >= 0, 0 = no step
+ * limit.  Host-side only: a step already enqueued keeps the limit it was launched with.  A handle that never calls it keeps the
+ * value of b2q_create. */
+int b2q_set_max_episode_steps(B2QHandle h, int max_episode_steps);
 
 #ifdef __cplusplus
 }

@@ -44,6 +44,12 @@ int b2q_sac_phase(B2QSacHandle h, int phase, const float* obs, const float* act,
  * eps [B,act_dim]: the N(0,1) draw of the student's sample().  losses_out device float[2] = {critic_loss, actor_loss}. */
 int b2q_sac_bc_learn(B2QSacHandle h, const float* obs, const float* ref_obs, int ref_obs_dim, B2QMlpHandle expert_actor, B2QMlpHandle expert_critic,
                      const float* eps, float* losses_out, void* stream);
+/* The same step with an optional eps: NULL draws the student's sample() noise from the counter RNG, Philox-4x32-10 keyed by
+ * seed + ctr * 0x9E3779B97F4A7C15 (ctr = the learner's device-side step counter, i.e. the number of completed learn / bc_learn steps),
+ * counter = (row, action) — the key rule of b2q_sac_learn's draws.  No noise tensor, and a CUDA-graph replay draws fresh noise every step.
+ * b2q_sac_bc_learn(..., eps, ...) == b2q_sac_bc_learn_seeded(..., eps, any seed, ...). */
+int b2q_sac_bc_learn_seeded(B2QSacHandle h, const float* obs, const float* ref_obs, int ref_obs_dim, B2QMlpHandle expert_actor,
+                            B2QMlpHandle expert_critic, const float* eps_or_null, uint64_t seed, float* losses_out, void* stream);
 /* the learner's own forward objects (0 actor, 1 twin critic, 2 target critic): always up to date with the parameters, so a
  * rollout can sample from the policy being trained without copying weights.  Owned by the learner. */
 B2QMlpHandle b2q_sac_mlp(B2QSacHandle h, int which);

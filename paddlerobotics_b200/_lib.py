@@ -32,6 +32,7 @@ SYMBOLS = {
     "b2q_set_state": (_i, [_vp, _vp, _vp]),
     "b2q_get_step_count": (_i, [_vp, _vp, _vp]),
     "b2q_launch_count": (C.c_int64, [_vp]),
+    "b2q_set_max_episode_steps": (_i, [_vp, _i]),
     # policy / critic MLP forward on wgmma tensor cores — include/b2q_mlp.h
     "b2q_mlp_create": (_i, [_i, _i, _i, _i, C.POINTER(_vp)]),
     "b2q_mlp_destroy": (_i, [_vp]),
@@ -50,6 +51,7 @@ SYMBOLS = {
     "b2q_sac_learn": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint64, _vp, _vp]),
     "b2q_sac_phase": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint64, _vp]),
     "b2q_sac_bc_learn": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "b2q_sac_bc_learn_seeded": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, C.c_uint64, _vp, _vp]),
     "b2q_sac_mlp": (_vp, [_vp, _i]),
     "b2q_sac_grad_ptr": (_vp, [_vp, _i]),
     "b2q_sac_loss_ptr": (_vp, [_vp]),
@@ -66,6 +68,8 @@ SYMBOLS = {
     "b2q_rpm_append_cursor": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "b2q_rpm_sample_cursor": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, C.c_uint64, _vp, _vp]),
     "b2q_rpm_append_masked_cursor": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u8p, _i, _i, _i, _i, _vp, _vp]),
+    "b2q_bc_observe": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _i, C.c_uint32, C.c_uint32, _i, _vp]),
+    "b2q_bc_gather_cursor": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     # camera images — include/b2q_render.h
     "b2q_render": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
 }

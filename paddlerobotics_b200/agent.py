@@ -355,11 +355,60 @@ class SACLearner:
             self.pull()
         return self.losses
 
+    def _bc_step(self, memory, expert, seed, acc):
+        """gather the next batch on the device cursor, one seeded BC update (counter-RNG noise), add its losses to acc."""
+        memory.gather_cursor(self._bc_perm, self._bc_cursor, self._bc_obs, self._bc_ref)
+        rc = self.lib.b2q_sac_bc_learn_seeded(self.h, self._bc_obs.data_ptr(), self._bc_ref.data_ptr(), self._bc_ref.shape[1], expert.actor.h,
+                                              expert.critic.h, None, C.c_uint64(seed), None, self._stream())
+        if rc != 0:
+            raise RuntimeError("b2q_sac_bc_learn_seeded: %d" % rc)
+        acc.add_(self.losses)
+
+    def bc_sweep(self, memory, expert, perm, n_batches, seed=0, graph_steps=64, pull=True):
+        """n_batches BC updates (BCtrain.py:132-136) on the batches perm[k B:(k + 1) B], k = 0 .. n_batches - 1, of `memory` (a
+        bc.BCReplayMemory), each one (device gather, b2q_sac_bc_learn_seeded with counter-RNG noise).  graph_steps G of them are captured
+        once into one CUDA graph and replayed n_batches // G times; the n_batches % G left over run eagerly, so no batch is added or
+        dropped.  No per-step host work, no per-step parameter pull: `pull` pulls once at the end.  Returns the device tensor [2] of the
+        mean (critic_loss, actor_loss) over the updates."""
+        dev, B = self.agent.device, self.batch
+        if getattr(self, "_bc_perm", None) is None or self._bc_perm.numel() < memory.max_size or self._bc_ref.shape[1] != memory.ref_obs.shape[1]:
+            self._bc_perm = torch.zeros(memory.max_size, dtype=torch.int64, device=dev)
+            self._bc_cursor = torch.zeros(1, dtype=torch.int64, device=dev)
+            self._bc_obs = torch.zeros(B, memory.obs.shape[1], device=dev)
+            self._bc_ref = torch.zeros(B, memory.ref_obs.shape[1], device=dev)
+            self._bc_acc = torch.zeros(2, device=dev)
+            self._bc_graphs = {}
+        assert perm.numel() >= n_batches * B
+        self._bc_perm[:perm.numel()].copy_(perm)
+        self._bc_cursor.zero_()
+        self._bc_acc.zero_()
+        G = max(1, int(graph_steps))
+        if n_batches >= G:
+            # the graph freezes every pointer it was captured with: key it by them
+            key = (G, memory.obs.data_ptr(), memory.ref_obs.data_ptr(), int(expert.actor.h.value), int(expert.critic.h.value), int(seed))
+            g = self._bc_graphs.get(key)
+            if g is None:
+                side = torch.cuda.Stream(device=dev)
+                side.wait_stream(torch.cuda.current_stream(dev))
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g, stream=side):
+                    for _ in range(G):
+                        self._bc_step(memory, expert, seed, self._bc_acc)
+                self._bc_graphs[key] = g
+            for _ in range(n_batches // G):
+                g.replay()
+        for _ in range(n_batches % G):
+            self._bc_step(memory, expert, seed, self._bc_acc)
+        if pull:
+            self.pull()
+        return self._bc_acc / max(n_batches, 1)
+
     def close(self):
         if getattr(self, "h", None):
             self.losses = self.losses.clone()      # the view of the learner's accumulators dies with the handle
             self._graph = None
             self._static = None
+            self._bc_graphs = None
             self.lib.b2q_sac_destroy(self.h)
             self.h = None
 

@@ -4,9 +4,12 @@ EnvWrapper.py:75-76) with sensor noise on rpy / drpy / q / qd (BCtrain.py:53-59)
 
     obs2noise(obs)            one row, NumPy global RNG, same draw order as the reference (bit-identical for one seed)
     obs2noise_batch(obs, gen) [N,49] device tensor, torch generator (the per-step path of the batched loop)
-    cal_agent_obs / cal_ref_obs, BCReplayMemory (device ring of (student obs, expert obs) pairs, BCreplay_buffer.py:21-84)
+    cal_agent_obs / cal_ref_obs, BCReplayMemory (device ring of (student obs, expert obs) pairs, BCreplay_buffer.py:21-84;
+                              observe / iter_pass: the fused noise + append kernel and the shuffled pass on a device cursor)
     run_bc(...)               collect with the student, clone from the expert with MujocoAgent.BClearn (alg/BC.py:53-72)
 """
+import ctypes as C
+
 import numpy as np
 import torch
 
@@ -67,6 +70,53 @@ class BCReplayMemory:
 
     def sample_batch_by_index(self, idx):
         return self.obs[idx], self.ref_obs[idx]
+
+    # ---- device path (b2q_bc_observe / b2q_bc_gather_cursor, include/b2q_rpm.h): float32 CUDA storage
+    def observe(self, obs, step, noise=True, append=True, seed=0):
+        """One control step in one launch: the student rows obs[:, 3:] + the sensor noise of BCtrain.py:53-59 (Philox key (seed, step),
+        counter (env row, expert column)), and with append=True the pairs (student row, obs row) at the ring's host cursor
+        (BCtrain.py:120).  obs: [N, 49] float32 CUDA tensor.  Returns the [N, 46] student rows."""
+        from . import _lib
+        obs = obs.contiguous()
+        n, d = obs.shape
+        assert obs.dtype == torch.float32 and obs.is_cuda and d == self.ref_obs.shape[1] and self.obs.shape[1] == d - 3
+        student = torch.empty(n, d - 3, device=obs.device, dtype=torch.float32)
+        ring = (self.obs.data_ptr(), self.ref_obs.data_ptr()) if append else (None, None)
+        rc = _lib.load().b2q_bc_observe(obs.data_ptr(), n, d, student.data_ptr(), *ring, self._pos, self.max_size, int(seed) & 0xFFFFFFFF,
+                                        int(step) & 0xFFFFFFFF, int(bool(noise)), C.c_void_p(torch.cuda.current_stream(obs.device).cuda_stream))
+        if rc != 0:
+            raise RuntimeError("b2q_bc_observe failed (%d)" % rc)
+        if append:
+            self._pos = (self._pos + n) % self.max_size
+            self._size = min(self.max_size, self._size + n)
+        return student
+
+    def gather_cursor(self, perm, cursor, out_obs, out_ref):
+        """Batch rows perm[cursor[0] + r] into out_obs / out_ref, then cursor[0] += batch (device int64 cursor: graph-capturable)."""
+        from . import _lib
+        rc = _lib.load().b2q_bc_gather_cursor(self.obs.data_ptr(), self.ref_obs.data_ptr(), perm.data_ptr(), perm.numel(), cursor.data_ptr(),
+                                              out_obs.data_ptr(), out_ref.data_ptr(), out_obs.shape[0], self.obs.shape[1], self.ref_obs.shape[1],
+                                              C.c_void_p(torch.cuda.current_stream(self.obs.device).cuda_stream))
+        if rc != 0:
+            raise RuntimeError("b2q_bc_gather_cursor failed (%d)" % rc)
+
+    def iter_pass(self, batch, size=None, generator=None):
+        """One shuffled pass of BCtrain.py:129-135 over the first `size` rows (default: all): a fresh device permutation and the batches
+        perm[j:j + batch] for j in range(0, size - batch, batch), gathered on the device cursor.  Yields (obs, ref_obs) static buffers
+        that the next batch overwrites."""
+        size = self._size if size is None else int(size)
+        dev = self.obs.device
+        perm = torch.randperm(size, device=dev, generator=generator)
+        cursor = torch.zeros(1, dtype=torch.int64, device=dev)
+        out = (torch.empty(batch, self.obs.shape[1], device=dev), torch.empty(batch, self.ref_obs.shape[1], device=dev))
+        for _ in pass_offsets(size, batch):
+            self.gather_cursor(perm, cursor, *out)
+            yield out
+
+
+def pass_offsets(size, batch):
+    """The batch offsets of one pass over `size` rows, BCtrain.py:132 (the last full batch is never taken, as in the reference)."""
+    return range(0, size - batch, batch)
 
 
 def run_bc(env, student, expert, etg_w, etg_b, iters, batch=1024, act_bound=0.3, warmup=0, train_every=1, sensor_noise=True, memory=200000, seed=0,

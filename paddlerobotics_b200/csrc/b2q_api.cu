@@ -193,6 +193,7 @@ struct EnvBase {
   virtual int get_state(void* out, cudaStream_t s) = 0;
   virtual int set_state(const void* in, cudaStream_t s) = 0;
   virtual int get_step_count(int32_t* out, cudaStream_t s) = 0;
+  virtual void set_max_steps(int m) = 0;
   virtual int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
                      int32_t* seg, cudaStream_t s) = 0;
 };
@@ -410,6 +411,7 @@ struct EnvT : EnvBase {
     CK(cudaMemcpyAsync(out, B.step_count, sizeof(int) * B.N, cudaMemcpyDeviceToDevice, s));
     return B2Q_OK;
   }
+  void set_max_steps(int m) override { cfg.max_episode_steps = m; kc.max_steps = m; }   // kc goes to the step kernel by value
   int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
              int32_t* seg, cudaStream_t s) override {
     if (!state || !env_ids || !view || !proj) { err = "b2q_render: null state, env_ids, view or proj"; return B2Q_EINVAL; }
@@ -481,6 +483,11 @@ int b2q_get_state(B2QHandle h, void* out, void* s) { return h ? h->impl->get_sta
 int b2q_set_state(B2QHandle h, const void* in, void* s) { return h ? h->impl->set_state(in, (cudaStream_t)s) : B2Q_EINVAL; }
 int b2q_get_step_count(B2QHandle h, int32_t* out, void* s) { return h ? h->impl->get_step_count(out, (cudaStream_t)s) : B2Q_EINVAL; }
 int64_t b2q_launch_count(B2QHandle h) { return h ? h->impl->launches : 0; }
+int b2q_set_max_episode_steps(B2QHandle h, int m) {
+  if (!h || m < 0) return B2Q_EINVAL;
+  h->impl->set_max_steps(m);
+  return B2Q_OK;
+}
 int b2q_render(B2QHandle h, const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int width, int height, uint8_t* rgba,
                float* depth, int32_t* seg, void* stream) {
   return h ? h->impl->render(state, env_ids, V, view, proj, width, height, rgba, depth, seg, (cudaStream_t)stream) : B2Q_EINVAL;

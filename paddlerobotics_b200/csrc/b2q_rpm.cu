@@ -1,7 +1,10 @@
-// b2q_rpm.cu — device replay memory kernels (include/b2q_rpm.h): batched ring append and uniform minibatch gather.
+// b2q_rpm.cu — device replay memory kernels (include/b2q_rpm.h): batched ring append and uniform minibatch gather; the behaviour-cloning
+// student observation (sensor noise + pair append) and the permutation gather on a device cursor.
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <cstdint>
 #include "../../include/b2q_rpm.h"
+#include "b2q_philox.cuh"
 
 namespace {
 __global__ void rpm_append_kernel(float* s_obs, float* s_act, float* s_rew, float* s_next, float* s_term, const float* obs, const float* act, const float* rew,
@@ -107,6 +110,43 @@ __global__ void __launch_bounds__(MASK_THREADS) rpm_advance_masked_kernel(long l
   const int m = block_sum(count_valid(valid, n), red);
   if (threadIdx.x == 0) { state[0] = (state[0] + m) % cap; state[1] = state[1] + m < cap ? state[1] + m : cap; }
 }
+
+// ---- behaviour cloning: student observation with sensor noise (+ optional ring append), and the permutation gather on a device cursor
+constexpr int BC_THREADS = 256;
+__device__ __forceinline__ float bc_sigma(int c) {      // BCtrain.py:55-58 over the sensor normalisers (bc.NOISE); 0 = no noise on column c
+  return c < 7 ? 0.f : c < 10 ? 0.6f : c < 13 ? 0.2f : c < 25 ? 0.1f : c < 37 ? 0.5f : 0.f;
+}
+// one thread per element of obs [n, D]: coalesced reads of the expert rows, coalesced writes of both ring rows and the student row
+__global__ void __launch_bounds__(BC_THREADS) bc_observe_kernel(const float* __restrict__ obs, int n, int D, float* __restrict__ student,
+    float* __restrict__ ring_obs, float* __restrict__ ring_ref, int pos, int cap, uint64_t key, int noise) {
+  const size_t total = (size_t)n * D;
+  for (size_t e = (size_t)blockIdx.x * BC_THREADS + threadIdx.x; e < total; e += (size_t)gridDim.x * BC_THREADS) {
+    const int i = (int)(e / D), c = (int)(e - (size_t)i * D);
+    const float o = obs[e];
+    const size_t slot = ring_ref ? (size_t)(((long long)pos + i) % cap) : 0;
+    if (ring_ref) ring_ref[slot * D + c] = o;
+    if (c < 3) continue;
+    const float sig = noise ? bc_sigma(c) : 0.f;
+    const float v = sig != 0.f ? __fadd_rn(o, __fmul_rn(sig, b2q_philox::philox_normal(key, (uint32_t)i, (uint32_t)c))) : o;
+    student[(size_t)i * (D - 3) + c - 3] = v;
+    if (ring_obs) ring_obs[slot * (D - 3) + c - 3] = v;
+  }
+}
+// one thread per element of the [batch, od + rd] gathered pair; state[0] is the pass offset
+__global__ void __launch_bounds__(BC_THREADS) bc_gather_kernel(const float* __restrict__ ring_obs, const float* __restrict__ ring_ref,
+    const int64_t* __restrict__ perm, int perm_len, const long long* __restrict__ state, float* __restrict__ out_obs, float* __restrict__ out_ref,
+    int batch, int od, int rd) {
+  const int w = od + rd;
+  const long long off = state[0];
+  for (int e = blockIdx.x * BC_THREADS + threadIdx.x; e < batch * w; e += gridDim.x * BC_THREADS) {
+    const int r = e / w, c = e - r * w;
+    if (off + r >= perm_len) continue;
+    const size_t src = (size_t)perm[off + r];
+    if (c < od) out_obs[(size_t)r * od + c] = ring_obs[src * od + c];
+    else out_ref[(size_t)r * rd + c - od] = ring_ref[src * rd + c - od];
+  }
+}
+__global__ void bc_cursor_advance_kernel(long long* state, int batch) { state[0] += batch; }
 }  // namespace
 
 extern "C" {
@@ -144,6 +184,24 @@ int b2q_rpm_append_masked_cursor(float* s_obs, float* s_act, float* s_rew, float
   rpm_append_masked_kernel<<<(n + tile - 1) / tile, MASK_THREADS, 0, (cudaStream_t)stream>>>(s_obs, s_act, s_rew, s_next, s_term, obs, act, rew, next_obs, term,
                                                                                             valid, n, od, ad, cap, tile, state);
   rpm_advance_masked_kernel<<<1, MASK_THREADS, 0, (cudaStream_t)stream>>>(state, valid, n, cap);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+int b2q_bc_observe(const float* obs, int n, int obs_dim, float* student, float* ring_obs, float* ring_ref, int pos, int cap, uint32_t seed, uint32_t step,
+                   int noise, void* stream) {
+  if (!obs || !student || n < 1 || obs_dim < 37 || (!ring_obs) != (!ring_ref)) return -1;
+  if (ring_ref && (cap < n || pos < 0)) return -1;
+  const size_t total = (size_t)n * obs_dim;
+  const int grid = (int)std::min<size_t>((total + BC_THREADS - 1) / BC_THREADS, 8192);
+  bc_observe_kernel<<<grid, BC_THREADS, 0, (cudaStream_t)stream>>>(obs, n, obs_dim, student, ring_obs, ring_ref, pos, cap,
+                                                                   (uint64_t)seed | ((uint64_t)step << 32), noise);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+int b2q_bc_gather_cursor(const float* ring_obs, const float* ring_ref, const int64_t* perm, int perm_len, long long* state, float* out_obs, float* out_ref,
+                         int batch, int obs_dim, int ref_dim, void* stream) {
+  if (!ring_obs || !ring_ref || !perm || !state || !out_obs || !out_ref || batch < 1 || obs_dim < 1 || ref_dim < 1 || perm_len < 0) return -1;
+  const int grid = std::min((batch * (obs_dim + ref_dim) + BC_THREADS - 1) / BC_THREADS, 4096);
+  bc_gather_kernel<<<grid, BC_THREADS, 0, (cudaStream_t)stream>>>(ring_obs, ring_ref, perm, perm_len, state, out_obs, out_ref, batch, obs_dim, ref_dim);
+  bc_cursor_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(state, batch);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 }

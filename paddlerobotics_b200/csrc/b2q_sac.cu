@@ -699,9 +699,11 @@ int b2q_sac_learn(B2QSacHandle s, const float* obs, const float* act, const floa
 }
 // Behaviour cloning of a (partial-observation) student from an expert (BC.BClearn, alg/BC.py:53-72): actor step on
 // -mean log N(expert_action | mean, std), then critic regression onto the expert's twin Q at the student's fresh sample.
-int b2q_sac_bc_learn(B2QSacHandle s, const float* obs, const float* ref_obs, int ref_obs_dim, B2QMlpHandle expert_actor, B2QMlpHandle expert_critic,
-                     const float* eps, float* losses_out, void* stream) {
-  if (!s || !obs || !ref_obs || !expert_actor || !expert_critic || !eps) return -1;
+// eps == NULL: the student's sample() draw comes from the counter RNG keyed by `seed` and the device step counter (the key of b2q_sac_learn's
+// draws), so the call needs no noise tensor and a CUDA-graph replay draws fresh noise every step.
+int b2q_sac_bc_learn_seeded(B2QSacHandle s, const float* obs, const float* ref_obs, int ref_obs_dim, B2QMlpHandle expert_actor, B2QMlpHandle expert_critic,
+                            const float* eps, uint64_t seed, float* losses_out, void* stream) {
+  if (!s || !obs || !ref_obs || !expert_actor || !expert_critic) return -1;
   cudaStream_t st = (cudaStream_t)stream;
   const int B = s->B, A = s->A, D = s->D, na = (int)s->an.n, nc = (int)(2 * s->cn.n);
   const Net& an = s->an;
@@ -716,7 +718,9 @@ int b2q_sac_bc_learn(B2QSacHandle s, const float* obs, const float* ref_obs, int
   if (actor_backward(s, st)) return -2;
   pdl_launch(k_adam_pack, dim3((na + 255) / 256), dim3(256), 0, st, s->p_actor, s->g_actor, s->m_a, s->v_a, na, s->lr_a, 0.9f, 0.999f, 1e-8f, s->d_step, (int*)nullptr, dst_of(s, NETS_ACTOR));
   // --- critic: a_now ~ pi_student(obs) (no grad); targets = expert Q(ref_obs, a_now)
-  if (b2q_mlp_forward(s->mlp_actor, obs, D, nullptr, B, B2Q_MLP_SAMPLE, 0, eps, s->cur_a, s->cur_logp, nullptr, st)) return -2;
+  // (the counter still holds the number of completed steps: only the critics' Adam below advances it)
+  if (b2q_mlp_forward_ex(s->mlp_actor, obs, D, nullptr, B, B2Q_MLP_SAMPLE, seed, eps, s->cur_a, s->cur_logp, nullptr, nullptr, nullptr,
+                         eps ? nullptr : s->d_step, st)) return -2;
   if (b2q_mlp_forward(expert_critic, ref_obs, ref_obs_dim, s->cur_a, B, B2Q_MLP_RAW, 0, nullptr, s->qn, nullptr, nullptr, st)) return -2;
   B2QMlpSaves sv = {nullptr /*x row-major: no consumer*/, s->xc_t, s->hc1_rm, s->hc1_t, s->hc2_rm, s->hc2_t};
   if (b2q_mlp_forward_ex(s->mlp_critic, obs, D, s->cur_a, B, B2Q_MLP_RAW, 0, nullptr, s->q, nullptr, nullptr, &sv, nullptr, nullptr, st)) return -2;
@@ -728,6 +732,11 @@ int b2q_sac_bc_learn(B2QSacHandle s, const float* obs, const float* ref_obs, int
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { s->err = cudaGetErrorString(e); return -2; }
   return 0;
+}
+int b2q_sac_bc_learn(B2QSacHandle s, const float* obs, const float* ref_obs, int ref_obs_dim, B2QMlpHandle expert_actor, B2QMlpHandle expert_critic,
+                     const float* eps, float* losses_out, void* stream) {
+  if (!eps) return -1;
+  return b2q_sac_bc_learn_seeded(s, obs, ref_obs, ref_obs_dim, expert_actor, expert_critic, eps, 0, losses_out, stream);
 }
 B2QMlpHandle b2q_sac_mlp(B2QSacHandle s, int which) { return !s ? nullptr : (which == 0 ? s->mlp_actor : (which == 1 ? s->mlp_critic : s->mlp_target)); }
 float* b2q_sac_grad_ptr(B2QSacHandle s, int which) { return !s ? nullptr : (which == 1 ? s->g_critic : s->g_actor); }   // which == 2: the flat bucket (starts at the actor part)

@@ -125,6 +125,11 @@ class VecQuadrupedalEnv:
     def launch_count(self):
         return int(self.lib.b2q_launch_count(self.h))
 
+    def set_max_episode_steps(self, m):
+        """The per-env episode step limit of every following step (0 = none); episodes already running keep their step count."""
+        _check(self.lib, self.h, self.lib.b2q_set_max_episode_steps(self.h, int(m)), "b2q_set_max_episode_steps")
+        self.cfg.max_episode_steps = int(m)
+
     def get_camera_image(self, width=640, height=480, env_ids=None, view=None, proj=None):
         """Ray-cast camera images of the current state (b2q_render, include/b2q_render.h): view v shows env env_ids[v] (default
         every env).  view / proj: [16] (one matrix for every view) or [V,16] column-major pybullet matrices; None = the follow
@@ -259,6 +264,61 @@ def _motor_mode(m):
     raise NotImplementedError("motor_control_mode %r: POSITION, TORQUE and HYBRID are provided (PWM raises in the reference's motor model too, laikago_motor.py:126-128)" % (m,))
 
 
+def quadrupedal_config(task="stairstair", motor_control_mode=None, sensor_mode=None, normal=1, reward_param=None, ETG=1, ETG_T=0.5, reward_p=5,
+                       random_param=None, ETG_H=20, vel_d=0.5, step_y=0.05, enable_action_filter=0, seed=0, terrain_param=None):
+    """The engine configuration of rlschool.make_env('Quadrupedal', ...) for any number of envs: (VecQuadrupedalEnv keywords including the
+    terrain's `heightfield`, the random_param flags).  Raises NotImplementedError for every option the engine does not provide."""
+    if ETG_H != ETG_H_CONST:
+        raise NotImplementedError("ETG_H must be %d (the RBF layer width is fixed in the kernel)" % ETG_H_CONST)
+    if task not in TASKS:
+        raise NotImplementedError("task %r is not provided (have: %s)" % (task, ", ".join(TASKS)))
+    sm = dict(SENSOR_MODE)
+    if sensor_mode:
+        unknown = set(sensor_mode) - set(SENSOR_MODE) - {"RNN"}
+        if unknown:
+            raise NotImplementedError("sensor_mode keys %s are not provided" % sorted(unknown))
+        sm.update({k: v for k, v in sensor_mode.items() if k != "RNN"})
+        rnn = sensor_mode.get("RNN")
+        if rnn and rnn.get("mode", "None") not in ("None", None):
+            raise NotImplementedError("sensor_mode['RNN'] mode %r: wrap the env with paddlerobotics_b200.obs_history.ObservationHistory instead" % (rnn.get("mode"),))
+    for k in _UNSUPPORTED_SENSORS:
+        if sm.get(k):
+            raise NotImplementedError("sensor_mode[%r]: this rlschool-only observation block is not provided (its layout is not in the reference tree)" % k)
+    rp = dict(Random_Param_Dict)
+    if random_param:
+        unknown = set(random_param) - set(Random_Param_Dict)
+        if unknown:
+            raise NotImplementedError("random_param keys %s are not provided" % sorted(unknown))
+        rp.update(random_param)
+    cfg = dict(etg_T=float(ETG_T), etg_T2=float(ETG_T), reward_p=float(reward_p), vel_d=float(vel_d), etg_enabled=int(bool(ETG)),
+               action_filter=int(bool(enable_action_filter)), motor_mode=_motor_mode(motor_control_mode),
+               sensor_dis=int(bool(sm["dis"])), sensor_contact=int(bool(sm["contact"])), sensor_imu=int(sm["imu"]), sensor_motor=int(sm["motor"]),
+               sensor_etg=int(bool(sm["ETG"])), obs_normal=int(bool(normal)), external_force=int(bool(rp["random_force"])),
+               stuck_termination=1, body_collisions=1, joint_limits=1, knee_contacts=1, noise_seed=int(seed))
+    if sm["noise"]:
+        cfg["noise_stdev"] = SENSOR_NOISE_STDDEV
+    if task == "balancebeam":
+        cfg["etg_foot_y_inset"] = float(step_y)
+    for k_ref, k_cfg in (("torso", "w_torso"), ("feet", "w_feet"), ("up", "w_up"), ("tau", "w_tau"), ("stand", "w_stand"),
+                         ("badfoot", "w_badfoot"), ("footcontact", "w_footcontact"), ("done", "w_done")):
+        if reward_param and k_ref in reward_param:
+            cfg[k_cfg] = float(reward_param[k_ref])
+    if reward_param and float(reward_param.get("stand", 0)) != 0:
+        raise NotImplementedError("reward_param['stand'] != 0: the stand term is not provided")
+    cfg["heightfield"] = make_terrain(task, step_y=float(step_y), **dict(terrain_param or {}))
+    return cfg, rp
+
+
+def etg_of_path(ETG_path, ETG_T=0.5):
+    """make_env's ETG_path rule: a `.npz` path gives its (w, b); anything else the default gait fit (train.py:298-299 defaults)."""
+    if ETG_path not in (None, "None", "") and str(ETG_path).endswith(".npz"):
+        z = np.load(ETG_path)
+        return z["w"], z["b"]
+    layer = ETG_layer(ETG_T, 0.026, ETG_H, 0.04, np.array([-np.pi / 2, 0]), 0.2, ETG_T)
+    w, b, _ = Opt_with_points(ETG=layer, ETG_T=ETG_T, Footheight=0.1, Steplength=0.05)
+    return w, b
+
+
 class QuadrupedalEnv:
     """N=1 mirror of the reference env object (numpy in/out): rlschool.make_env('Quadrupedal', ...) of ETGRL/train.py:305-309.
     Every keyword of that call is honoured or raises NotImplementedError — nothing is swallowed."""
@@ -268,60 +328,20 @@ class QuadrupedalEnv:
                  step_y=0.05, enable_action_filter=0, device=0, precision="f32", seed=0, terrain_param=None, **engine_cfg):
         if render:
             raise NotImplementedError("render=True: there is no GUI / camera on the GPU path")
-        if ETG_H != ETG_H_CONST:
-            raise NotImplementedError("ETG_H must be %d (the RBF layer width is fixed in the kernel)" % ETG_H_CONST)
-        if task not in TASKS:
-            raise NotImplementedError("task %r is not provided (have: %s)" % (task, ", ".join(TASKS)))
-        sm = dict(SENSOR_MODE)
-        if sensor_mode:
-            unknown = set(sensor_mode) - set(SENSOR_MODE) - {"RNN"}
-            if unknown:
-                raise NotImplementedError("sensor_mode keys %s are not provided" % sorted(unknown))
-            sm.update({k: v for k, v in sensor_mode.items() if k != "RNN"})
-            rnn = sensor_mode.get("RNN")
-            if rnn and rnn.get("mode", "None") not in ("None", None):
-                raise NotImplementedError("sensor_mode['RNN'] mode %r: wrap the env with paddlerobotics_b200.obs_history.ObservationHistory instead" % (rnn.get("mode"),))
-        for k in _UNSUPPORTED_SENSORS:
-            if sm.get(k):
-                raise NotImplementedError("sensor_mode[%r]: this rlschool-only observation block is not provided (its layout is not in the reference tree)" % k)
-        rp = dict(Random_Param_Dict)
-        if random_param:
-            unknown = set(random_param) - set(Random_Param_Dict)
-            if unknown:
-                raise NotImplementedError("random_param keys %s are not provided" % sorted(unknown))
-            rp.update(random_param)
+        cfg, rp = quadrupedal_config(task=task, motor_control_mode=motor_control_mode, sensor_mode=sensor_mode, normal=normal, reward_param=reward_param,
+                                     ETG=ETG, ETG_T=ETG_T, reward_p=reward_p, random_param=random_param, ETG_H=ETG_H, vel_d=vel_d, step_y=step_y,
+                                     enable_action_filter=enable_action_filter, seed=seed, terrain_param=terrain_param)
         self._random_dynamics, self._random_force = bool(rp["random_dynamics"]), bool(rp["random_force"])
         self._rng = np.random.default_rng(seed)
-        cfg = dict(etg_T=float(ETG_T), etg_T2=float(ETG_T), reward_p=float(reward_p), vel_d=float(vel_d), etg_enabled=int(bool(ETG)),
-                   action_filter=int(bool(enable_action_filter)), motor_mode=_motor_mode(motor_control_mode),
-                   sensor_dis=int(bool(sm["dis"])), sensor_contact=int(bool(sm["contact"])), sensor_imu=int(sm["imu"]), sensor_motor=int(sm["motor"]),
-                   sensor_etg=int(bool(sm["ETG"])), obs_normal=int(bool(normal)), external_force=int(self._random_force),
-                   stuck_termination=1, body_collisions=1, joint_limits=1, knee_contacts=1, noise_seed=int(seed))
-        if sm["noise"]:
-            cfg["noise_stdev"] = SENSOR_NOISE_STDDEV
-        if task == "balancebeam":
-            cfg["etg_foot_y_inset"] = float(step_y)
-        for k_ref, k_cfg in (("torso", "w_torso"), ("feet", "w_feet"), ("up", "w_up"), ("tau", "w_tau"), ("stand", "w_stand"),
-                             ("badfoot", "w_badfoot"), ("footcontact", "w_footcontact"), ("done", "w_done")):
-            if reward_param and k_ref in reward_param:
-                cfg[k_cfg] = float(reward_param[k_ref])
-        if reward_param and float(reward_param.get("stand", 0)) != 0:
-            raise NotImplementedError("reward_param['stand'] != 0: the stand term is not provided")
+        hf = cfg.pop("heightfield")
         cfg.update(engine_cfg)
-        tp = dict(terrain_param or {})
-        hf = make_terrain(task, step_y=float(step_y), **tp)
         self.task = task
         self.vec = VecQuadrupedalEnv(1, device=device, precision=precision, heightfield=hf, **cfg)
         self._dyn_row = dynamic_dict_to_row(dynamic_param) if dynamic_param else None
         if self._dyn_row is not None:
             self.vec.set_dynamics(self._dyn_row[None, :])
         self.observation_space, self.action_space = _Space(self.vec.observation_dim), _Space(self.vec.action_dim)
-        layer = ETG_layer(ETG_T, 0.026, ETG_H, 0.04, np.array([-np.pi / 2, 0]), 0.2, ETG_T)
-        if ETG_path not in (None, "None", "") and str(ETG_path).endswith(".npz"):
-            z = np.load(ETG_path)
-            self._w, self._b = z["w"], z["b"]
-        else:
-            self._w, self._b, _ = Opt_with_points(ETG=layer, ETG_T=ETG_T, Footheight=0.1, Steplength=0.05)  # train.py:298-299 defaults
+        self._w, self._b = etg_of_path(ETG_path, ETG_T)
 
     def reset(self, ETG_w=None, ETG_b=None, x_noise=0, hardset=None, dynamic_param=None):
         if hardset is not None:

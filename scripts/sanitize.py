@@ -97,5 +97,16 @@ big.sync_host()
 # ES fitness with 33 rollouts per individual: lane 0 runs the strided loop twice
 evr = PopulationEvaluator(3, 33, max_steps=2)
 evr.evaluate(np.repeat(w[None], 3, 0), np.repeat(b[None], 3, 0))
+# behaviour cloning: student observation with noise into a ring that wraps (capacity not a multiple of n), without a ring; the gather cursor
+# past the end of its permutation; bc_sweep with graph replays and an eager remainder (counter-RNG BC update)
+from paddlerobotics_b200.bc import BCReplayMemory
+bcm = BCReplayMemory(1001, 46, 49)
+bcm._pos = 700
+bcm.observe(torch.randn(513, 49, device="cuda"), 3)
+bcm.observe(torch.randn(37, 49, device="cuda"), 4, noise=False, append=False)
+bcur = torch.tensor([1001 - 20], dtype=torch.int64, device="cuda")
+bcm.gather_cursor(torch.randperm(1001, device="cuda"), bcur, torch.empty(128, 46, device="cuda"), torch.empty(128, 49, device="cuda"))
+bcl = SACLearner(MujocoAgent(46, 12, seed=4), 128)
+bcl.bc_sweep(bcm, expert, torch.randperm(1001, device="cuda"), 7, seed=1, graph_steps=3)
 torch.cuda.synchronize()
 print("sanitizer script done")
