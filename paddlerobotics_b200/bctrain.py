@@ -23,8 +23,7 @@ import torch
 
 from . import bc
 from .agent import MujocoAgent, SACLearner
-from .env import VecQuadrupedalEnv, etg_of_path, quadrupedal_config
-from .etg import dynamic_dict_to_row, param2dynamic_dict
+from .env import VecQuadrupedalEnv, apply_dynamic_param, etg_of_path, quadrupedal_config
 from .train import EVAL_TERMS
 
 ACTOR_LR, CRITIC_LR = 3e-4, 3e-4            # BCtrain.py:44-45
@@ -150,10 +149,7 @@ def env_kwargs(args):
 
 def make_vec_env(args, n, auto_reset, max_episode_steps=0):
     env = VecQuadrupedalEnv(n, auto_reset=auto_reset, max_episode_steps=max_episode_steps, **env_kwargs(args))
-    if args.dynamic_param:
-        row = dynamic_dict_to_row(param2dynamic_dict(np.load(args.dynamic_param).reshape(-1)))
-        env.set_dynamics(np.repeat(row[None], n, 0))
-    return env
+    return apply_dynamic_param(env, args.dynamic_param)
 
 
 def run_episodes(env, policy, w, b, act_bound, max_step, x_noise=0, render=None):

@@ -309,6 +309,15 @@ def quadrupedal_config(task="stairstair", motor_control_mode=None, sensor_mode=N
     return cfg, rp
 
 
+def apply_dynamic_param(env, path):
+    """A command's --dynamic_param: PATH.npy holds a 48-vector in [-1, 1] (a dynamic_param{epoch}.npy of dynamic_train) that goes through
+    param2dynamic_dict to every env of `env`; an empty path keeps the nominal dynamics.  Returns env."""
+    if path:
+        row = dynamic_dict_to_row(param2dynamic_dict(np.load(path).reshape(-1)))
+        env.set_dynamics(np.repeat(row[None], env.num_envs, 0))
+    return env
+
+
 def etg_of_path(ETG_path, ETG_T=0.5):
     """make_env's ETG_path rule: a `.npz` path gives its (w, b); anything else the default gait fit (train.py:298-299 defaults)."""
     if ETG_path not in (None, "None", "") and str(ETG_path).endswith(".npz"):

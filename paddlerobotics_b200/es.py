@@ -98,6 +98,215 @@ class SimpleGA:
         return (self.best_param, self.best_reward, self.curr_best_reward, self.sigma)
 
 
+# ---- the gradient-style solvers of dynamics identification (Dynamic_parallel_model.py:102-149; ETGRL/alg/es.py:145-211,328-619).
+#      Each keeps the reference's arithmetic order and dtypes, so an identically seeded run asks identical populations: the ranks are
+#      float32, the Adam moments start as float32, and OpenES / PEPG move mu twice per tell (once directly, once through Adam).
+
+def compute_centered_ranks(x):
+    """Ranks of x (0 = smallest) mapped to [-0.5, 0.5] in float32; ties are broken by np.argsort's default order."""
+    ranks = np.empty(x.size, dtype=int)
+    ranks[x.ravel().argsort()] = np.arange(x.size)
+    y = ranks.reshape(x.shape).astype(np.float32)
+    y /= (x.size - 1)
+    y -= .5
+    return y
+
+
+class Adam:
+    """Adam ascent on `pi.mu`: update(g) moves pi.mu by -a·m/(sqrt(v)+eps) with the bias-corrected step a (beta1 0.99, beta2 0.999)."""
+
+    def __init__(self, pi, stepsize, beta1=0.99, beta2=0.999, epsilon=1e-08):
+        self.pi, self.stepsize, self.beta1, self.beta2, self.epsilon = pi, stepsize, beta1, beta2, epsilon
+        self.t = 0
+        self.m = np.zeros(pi.num_params, dtype=np.float32)
+        self.v = np.zeros(pi.num_params, dtype=np.float32)
+
+    def update(self, g):
+        self.t += 1
+        a = self.stepsize * np.sqrt(1 - self.beta2 ** self.t) / (1 - self.beta1 ** self.t)
+        self.m = self.beta1 * self.m + (1 - self.beta1) * g
+        self.v = self.beta2 * self.v + (1 - self.beta2) * (g * g)
+        self.pi.mu = self.pi.mu + (-a * self.m / (np.sqrt(self.v) + self.epsilon))
+
+
+class SimpleES:
+    """Gaussian search around mu; tell() moves mu to the softmax(3·normalised reward)-weighted mean of the population."""
+
+    def __init__(self, num_params, popsize=256, sigma_init=0.1, sigma_decay=0.999, sigma_limit=0.01, weight_decay=0.01, param=None):
+        self.num_params, self.popsize = num_params, popsize
+        self.sigma, self.sigma_decay, self.sigma_limit, self.weight_decay = sigma_init, sigma_decay, sigma_limit, weight_decay
+        self.mu = np.zeros(num_params) if param is None else param
+        self.best_mu = np.zeros(num_params) if param is None else param
+        self.best_reward = 0
+        self.first_iteration = True
+
+    def ask(self):
+        self.epsilon = np.random.randn(self.popsize, self.num_params)
+        self.solutions = self.mu.reshape(1, self.num_params) + self.epsilon * self.sigma
+        return self.solutions
+
+    def tell(self, reward_table_result):
+        assert len(reward_table_result) == self.popsize, "Inconsistent reward_table size reported."
+        reward = np.array(reward_table_result)
+        if self.weight_decay > 0:
+            reward += compute_weight_decay(self.weight_decay, self.solutions)
+        top = np.argsort(reward)[::-1][0]
+        self.curr_best_reward, self.curr_best_mu = reward[top], self.solutions[top]
+        if self.first_iteration or self.curr_best_reward > self.best_reward:
+            self.first_iteration = False
+            self.best_reward, self.best_mu = self.curr_best_reward, self.curr_best_mu
+        if self.sigma > self.sigma_limit:
+            self.sigma *= self.sigma_decay
+        lo, spread = np.min(reward), np.max(reward) - np.min(reward)
+        if spread > 1e-2:
+            reward = 3 * (reward - lo) / spread
+        e = np.exp(reward)
+        weight = e / np.sum(e)
+        self.mu = np.zeros(self.num_params)
+        for i in range(self.popsize):               # sequential sum: the reference's order of additions
+            self.mu += weight[i] * self.solutions[i]
+
+    def result(self):
+        return (self.best_mu, self.best_reward, self.curr_best_reward, self.sigma)
+
+
+class OpenES:
+    """OpenAI-ES: a Gaussian population around mu and a normalised-reward gradient step on mu."""
+
+    def __init__(self, num_params, sigma_init=0.1, sigma_decay=0.999, sigma_limit=0.01, learning_rate=0.01, learning_rate_decay=0.9999,
+                 learning_rate_limit=0.001, popsize=256, antithetic=False, weight_decay=0.01, rank_fitness=True, forget_best=True):
+        self.num_params, self.popsize = num_params, popsize
+        self.sigma, self.sigma_init, self.sigma_decay, self.sigma_limit = sigma_init, sigma_init, sigma_decay, sigma_limit
+        self.learning_rate, self.learning_rate_decay, self.learning_rate_limit = learning_rate, learning_rate_decay, learning_rate_limit
+        self.antithetic = antithetic
+        if antithetic:
+            assert popsize % 2 == 0, "Population size must be even"
+            self.half_popsize = popsize // 2
+        self.mu = np.zeros(num_params)
+        self.best_mu = np.zeros(num_params)
+        self.best_reward = 0
+        self.first_iteration = True
+        self.weight_decay, self.rank_fitness = weight_decay, rank_fitness
+        self.forget_best = True if rank_fitness else forget_best
+        self.optimizer = Adam(self, learning_rate)
+
+    def ask(self):
+        if self.antithetic:
+            half = np.random.randn(self.half_popsize, self.num_params)
+            self.epsilon = np.concatenate([half, -half])
+        else:
+            self.epsilon = np.random.randn(self.popsize, self.num_params)
+        self.solutions = self.mu.reshape(1, self.num_params) + self.epsilon * self.sigma
+        return self.solutions
+
+    def tell(self, reward_table_result):
+        assert len(reward_table_result) == self.popsize, "Inconsistent reward_table size reported."
+        reward = np.array(reward_table_result)
+        if self.rank_fitness:
+            reward = compute_centered_ranks(reward)
+        if self.weight_decay > 0:
+            reward += compute_weight_decay(self.weight_decay, self.solutions)
+        top = np.argsort(reward)[::-1][0]
+        self.curr_best_reward, self.curr_best_mu = reward[top], self.solutions[top]
+        if self.first_iteration or self.forget_best or self.curr_best_reward > self.best_reward:
+            self.first_iteration = False
+            self.best_reward, self.best_mu = self.curr_best_reward, self.curr_best_mu
+        normalized = (reward - np.mean(reward)) / np.std(reward)
+        change_mu = 1. / (self.popsize * self.sigma) * np.dot(self.epsilon.T, normalized)
+        self.mu += self.learning_rate * change_mu
+        self.optimizer.stepsize = self.learning_rate
+        self.optimizer.update(-change_mu)
+        if self.sigma > self.sigma_limit:
+            self.sigma *= self.sigma_decay
+        if self.learning_rate > self.learning_rate_limit:
+            self.learning_rate *= self.learning_rate_decay
+
+    def result(self):
+        return (self.best_mu, self.best_reward, self.curr_best_reward, self.sigma)
+
+
+class PEPG:
+    """Parameter-exploring policy gradients: antithetic pairs mu ± eps with a per-parameter sigma that adapts, each step clipped to
+    ±sigma_max_change·sigma; with elite_ratio > 0, mu moves by the mean offset of the elite instead of the Adam step."""
+
+    def __init__(self, num_params, sigma_init=0.10, sigma_alpha=0.20, sigma_decay=0.999, sigma_limit=0.01, sigma_max_change=0.2, learning_rate=0.01,
+                 learning_rate_decay=0.9999, learning_rate_limit=0.01, elite_ratio=0, popsize=256, average_baseline=True, weight_decay=0.01,
+                 rank_fitness=True, forget_best=True):
+        self.num_params, self.popsize = num_params, popsize
+        self.sigma_init, self.sigma_alpha, self.sigma_decay, self.sigma_limit, self.sigma_max_change = sigma_init, sigma_alpha, sigma_decay, sigma_limit, sigma_max_change
+        self.learning_rate, self.learning_rate_decay, self.learning_rate_limit = learning_rate, learning_rate_decay, learning_rate_limit
+        self.average_baseline = average_baseline
+        if average_baseline:
+            assert popsize % 2 == 0, "Population size must be even"
+            self.batch_size = popsize // 2
+        else:
+            assert popsize & 1, "Population size must be odd"
+            self.batch_size = (popsize - 1) // 2
+        self.elite_popsize = int(popsize * elite_ratio)
+        self.use_elite = self.elite_popsize > 0
+        self.mu = np.zeros(num_params)
+        self.sigma = np.ones(num_params) * sigma_init
+        self.best_mu = np.zeros(num_params)
+        self.best_reward = 0
+        self.first_iteration = True
+        self.weight_decay, self.rank_fitness = weight_decay, rank_fitness
+        self.forget_best = True if rank_fitness else forget_best
+        self.optimizer = Adam(self, learning_rate)
+
+    def ask(self):
+        self.epsilon = np.random.randn(self.batch_size, self.num_params) * self.sigma.reshape(1, self.num_params)
+        self.epsilon_full = np.concatenate([self.epsilon, -self.epsilon])
+        eps = self.epsilon_full if self.average_baseline else np.concatenate([np.zeros((1, self.num_params)), self.epsilon_full])
+        self.solutions = self.mu.reshape(1, self.num_params) + eps      # without the average baseline, member 0 is mu itself
+        return self.solutions
+
+    def tell(self, reward_table_result):
+        assert len(reward_table_result) == self.popsize, "Inconsistent reward_table size reported."
+        table = np.array(reward_table_result)
+        if self.rank_fitness:
+            table = compute_centered_ranks(table)
+        if self.weight_decay > 0:
+            table += compute_weight_decay(self.weight_decay, self.solutions)
+        if self.average_baseline:
+            base, reward = np.mean(table), table
+        else:
+            base, reward = table[0], table[1:]
+        idx = np.argsort(reward)[::-1]
+        if self.use_elite:
+            idx = idx[0:self.elite_popsize]
+        if self.average_baseline or reward[idx[0]] > base:
+            self.curr_best_mu, self.curr_best_reward = self.mu + self.epsilon_full[idx[0]], reward[idx[0]]
+        else:
+            self.curr_best_mu, self.curr_best_reward = self.mu, base
+        if self.first_iteration:
+            self.sigma = np.ones(self.num_params) * self.sigma_init
+        if self.first_iteration or self.forget_best or self.curr_best_reward > self.best_reward:
+            self.first_iteration = False
+            self.best_mu, self.best_reward = self.curr_best_mu, self.curr_best_reward
+        eps, sigma = self.epsilon, self.sigma
+        if self.use_elite:
+            self.mu += self.epsilon_full[idx].mean(axis=0)
+        else:
+            change_mu = np.dot(reward[:self.batch_size] - reward[self.batch_size:], eps)
+            self.optimizer.stepsize = self.learning_rate
+            self.optimizer.update(-change_mu)
+            self.mu += change_mu * self.learning_rate
+        if self.sigma_alpha > 0:
+            stdev_reward = 1.0 if self.rank_fitness else reward.std()
+            S = (eps * eps - (sigma * sigma).reshape(1, self.num_params)) / sigma.reshape(1, self.num_params)
+            rS = (reward[:self.batch_size] + reward[self.batch_size:]) / 2.0 - base
+            change = self.sigma_alpha * (np.dot(rS, S) / (2 * self.batch_size * stdev_reward))
+            change = np.maximum(np.minimum(change, self.sigma_max_change * self.sigma), -self.sigma_max_change * self.sigma)
+            self.sigma += change
+        if self.sigma_decay < 1:
+            self.sigma[self.sigma > self.sigma_limit] *= self.sigma_decay
+        if self.learning_rate_decay < 1 and self.learning_rate > self.learning_rate_limit:
+            self.learning_rate *= self.learning_rate_decay
+
+    def result(self):
+        return (self.best_mu, self.best_reward, self.curr_best_reward, self.sigma)
+
+
 def shard_range(n, rank, world):
     """Contiguous shard [lo, hi) of n units owned by `rank` (SURVEY §8e: GPU g owns [g·N/G,(g+1)·N/G))."""
     return (n * rank) // world, (n * (rank + 1)) // world
@@ -272,8 +481,8 @@ class DynamicsEvaluator:
         """solutions [pop,48] in [-1,1] (identical on every rank) -> reward [pop] = mean over the gait keys (identical on every rank);
         DIVERGED_REWARD for an individual whose rollout is non-finite."""
         import torch
-        from .etg import dynamic_dict_to_row, param2dynamic_dict
-        rows = np.array([dynamic_dict_to_row(param2dynamic_dict(np.asarray(s))) for s in np.asarray(solutions)[self.lo:self.hi]])
+        from .etg import param2dynamic_rows
+        rows = param2dynamic_rows(np.asarray(solutions)[self.lo:self.hi])          # the rows of param2dynamic_dict, bit for bit
         env = self.env
         env.set_dynamics(np.tile(rows, (len(self.keys), 1)))          # env.reset(hardset=False, dynamic_param=...) :55
         env.reset()

@@ -211,3 +211,21 @@ def dynamic_dict_to_row(d=None, latency_unit_s=1e-3):
         if "legmass" in d: row[33:36] = d["legmass"]
         if "leginertia" in d: row[36:48] = d["leginertia"]
     return row
+
+
+def param2dynamic_rows(params):
+    """[P,48] vectors in [-1,1] -> [P,48] engine rows: dynamic_dict_to_row(param2dynamic_dict(p)) for every p at once, with the same
+    elementwise operations in the same order, so every row is bit-identical to the per-vector one."""
+    p = np.clip(np.asarray(params, dtype=np.float64).reshape(-1, 48), -1, 1)
+    kd0 = np.array([1., 2., 2.] * 4)
+    rows = np.empty((p.shape[0], 48))
+    rows[:, 0:12] = np.clip(80 * np.ones(12) + 40 * p[:, 21:33], 20, 200)
+    rows[:, 12:24] = np.clip(kd0 + p[:, 33:45] * np.array([1, 2, 2] * 4), 0, 5)
+    rows[:, 24] = np.clip(0.2 + 10 * p[:, 1], 0, 20)
+    rows[:, 25] = np.clip(40 + 10 * p[:, 0], 0, 80) * 1e-3
+    rows[:, 26:29] = np.clip(np.array([0, 0, -10]) + p[:, 45:48] * np.array([2, 2, 10]), np.array([-5, -5, -20]), np.array([5, 5, -4]))
+    rows[:, 29] = np.clip(1.5 + 1 * p[:, 2], 0.5, 3)
+    rows[:, 30:33] = np.clip(np.ones(3) + 1 * p[:, 3:6], 0.1, 3)
+    rows[:, 33:36] = np.clip(np.ones(3) + 1 * p[:, 6:9], 0.1, 3)
+    rows[:, 36:48] = np.clip(np.ones(12) + 1 * p[:, 9:21], 0.1, 3)
+    return rows

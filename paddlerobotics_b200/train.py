@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from .agent import MujocoAgent, SACLearner
-from .env import VecQuadrupedalEnv
+from .env import VecQuadrupedalEnv, apply_dynamic_param
 from .es import PopulationEvaluator, SimpleGA, solutions_to_etg_device
 from .etg import ETG_layer, Opt_with_points
 from .replay import ReplayMemory
@@ -23,7 +23,7 @@ from .terrain import make_terrain
 GAMMA, TAU, ALPHA, ACTOR_LR, CRITIC_LR = 0.99, 0.005, 0.2, 3e-4, 3e-4     # train.py:43-47
 
 
-def main(argv=None):
+def parser():
     p = argparse.ArgumentParser()
     p.add_argument("--num_envs", type=int, default=4096)
     p.add_argument("--max_steps", type=int, default=400000, help="total env steps (all envs)")
@@ -62,22 +62,44 @@ def main(argv=None):
     p.add_argument("--render_dir", type=str, default="", help="--eval: write env 0's camera image of every step to DIR/img{step}.png (train.py:196-199); empty = no frames")
     p.add_argument("--render_width", type=int, default=640)
     p.add_argument("--render_height", type=int, default=480)
+    p.add_argument("--dynamic_param", type=str, default="", help="PATH.npy: a 48-vector in [-1, 1] (dynamic_train's dynamic_param{epoch}.npy) -> "
+                   "param2dynamic_dict -> every env of training, the ES phase and --eval (train.py:302-303); empty = nominal dynamics")
+    return p
+
+
+def env_config(args):
+    """The reward weights of the command line (train.py:255-261) go to BOTH the training env and the ES evaluator: ES must optimise the
+    reward SAC is trained on."""
+    return dict(w_torso=args.torso, w_feet=args.feet, w_up=args.up, w_tau=args.tau, w_badfoot=args.badfoot, w_footcontact=args.footcontact,
+                heightfield=make_terrain(args.task_mode, step_y=args.step_y), stuck_termination=1, body_collisions=1,
+                etg_foot_y_inset=args.step_y if args.task_mode == "balancebeam" else 0.0)
+
+
+def make_envs(args, env_cfg, policy=None):
+    """The training env and the ES phase's PopulationEvaluator (None without --ES), both on the --dynamic_param dynamics."""
+    env = apply_dynamic_param(VecQuadrupedalEnv(args.num_envs, auto_reset=True, max_episode_steps=args.e_step, **env_cfg), args.dynamic_param)
+    evaluator = None
+    if args.ES:
+        evaluator = PopulationEvaluator(args.popsize, args.es_rollouts, max_steps=args.e_step, policy=policy, act_bound=args.act_bound, **env_cfg)
+        apply_dynamic_param(evaluator.env, args.dynamic_param)
+    return env, evaluator
+
+
+def main(argv=None):
+    p = parser()
     args = p.parse_args(argv)
     torch.manual_seed(args.seed); np.random.seed(args.seed)
     n = args.num_envs
     layer = ETG_layer(args.ETG_T, 0.026, 20, 0.04, np.array([-np.pi / 2, 0]), 0.2, args.ETG_T)
     w0, b0, prior_points = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, Footheight=args.footheight, Steplength=args.steplen)     # train.py:298-299
     w, b = w0, b0
-    # the reward weights of the command line (train.py:255-261) go to BOTH the training env and the ES evaluator: ES must optimise the
-    # reward SAC is trained on
-    env_cfg = dict(w_torso=args.torso, w_feet=args.feet, w_up=args.up, w_tau=args.tau, w_badfoot=args.badfoot, w_footcontact=args.footcontact,
-                   heightfield=make_terrain(args.task_mode, step_y=args.step_y), stuck_termination=1, body_collisions=1,
-                   etg_foot_y_inset=args.step_y if args.task_mode == "balancebeam" else 0.0)
+    env_cfg = env_config(args)
     if args.eval:
         if not args.load:
             p.error("--eval 1 evaluates a checkpoint: it needs --load itr_*.pt")
         return evaluate(args, env_cfg)
-    env = VecQuadrupedalEnv(n, auto_reset=True, max_episode_steps=args.e_step, **env_cfg)
+    # the evaluator's policy reads `learner` when it runs, so it may be built before the learner
+    env, evaluator = make_envs(args, env_cfg, policy=lambda o: learner.actor.forward(o)[0][0])
     agent = MujocoAgent(49, 12, seed=args.seed)
     ETG_best_param = np.zeros(12)                                                                                                 # ES_solver.get_best_param(), train.py:348
     if args.load:
@@ -93,8 +115,6 @@ def main(argv=None):
     rpm = ReplayMemory(args.memory, 49, 12, device_cursor=bool(args.graph_iter and args.overlap))
     solver = SimpleGA(12, sigma_init=args.sigma, sigma_decay=args.sigma_decay, sigma_limit=0.005, elite_ratio=0.1, weight_decay=0.005,
                       popsize=args.popsize, param=ETG_best_param.copy())                                                          # train.py:288-295
-    evaluator = PopulationEvaluator(args.popsize, args.es_rollouts, max_steps=args.e_step, policy=lambda o: learner.actor.forward(o)[0][0],
-                                    act_bound=args.act_bound, **env_cfg) if args.ES else None
     obs = env.reset(w, b).clone()
     total, it, last_es, t0 = 0, 0, 0, time.perf_counter()
     s_learn = torch.cuda.Stream(device=env.device)
@@ -236,7 +256,7 @@ def evaluate(args, env_cfg):
     z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
     w, b = z["w"], z["b"]
     n = args.eval_envs
-    env = VecQuadrupedalEnv(n, auto_reset=False, **env_cfg)
+    env = apply_dynamic_param(VecQuadrupedalEnv(n, auto_reset=False, **env_cfg), args.dynamic_param)
     lib, dev, es, stream = _lib.load(), env.device, env.obs.element_size(), env._stream()
     if args.render_dir:
         os.makedirs(args.render_dir, exist_ok=True)
