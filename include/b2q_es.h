@@ -14,6 +14,19 @@ extern "C" {
 #endif
 /* per control step: for alive envs ret += reward, len += 1, alive &= !done.  elem_size 4 (float) or 8 (double). */
 int b2q_es_accumulate(const void* reward, const uint8_t* done, uint8_t* alive, void* ret, int32_t* len, int n, int elem_size, void* stream);
+/* The per-episode statistics of an evaluation (pretrain.py:135-154 run_episode, train.py:202-207 run_evaluate_episodes) in ONE launch per
+ * control step.  For every env i that is still alive:
+ *   ret[i] += reward[i]; len[i] += 1                                     (bit-identical to b2q_es_accumulate)
+ *   term_sum[j*n + i] += info[i*info_dim + cols[j]]     for j < ncols   (per-term episode sums, NaN propagates)
+ *   count[i] += info[i*info_dim + count_col] >= thresh                  (when count_col >= 0; NaN does not count)
+ *   alive[i] &= !done[i]
+ * cols: HOST array of ncols (0..B2Q_ES_MAX_TERMS) info columns, copied by value into the kernel arguments: no device allocation, so the
+ * call can be captured in a CUDA graph.  count_col = -1: no count, count may be NULL.  info / term_sum may be NULL when unused.
+ * Returns -1 for a NULL required pointer, ncols out of range or a column outside [0, info_dim); -2 on a launch error. */
+#define B2Q_ES_MAX_TERMS 16
+int b2q_es_accumulate_terms(const void* reward, const uint8_t* done, uint8_t* alive, void* ret, int32_t* len, const void* info, int info_dim,
+                            const int32_t* cols, int ncols, void* term_sum, int count_col, double thresh, int32_t* count, int n, int elem_size,
+                            void* stream);
 /* fitness[i] = mean over the individual's rollouts of ret; mean_len (may be NULL) likewise for episode lengths. */
 int b2q_es_fitness(const void* ret, const int32_t* len, void* fitness, void* mean_len, int pop, int rollouts, int elem_size, void* stream);
 /* Batched ETG fit (SURVEY §8f-1): for each individual i, points = prior_points + solutions[i].reshape(6,2) and

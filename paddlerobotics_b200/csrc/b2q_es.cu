@@ -20,6 +20,27 @@ __global__ void es_accumulate_kernel(const T* __restrict__ reward, const uint8_t
   }
 }
 
+struct TermCols { int32_t c[B2Q_ES_MAX_TERMS]; };   // by value in the kernel's parameter space
+
+// es_accumulate_kernel plus the per-term sums and the success count of the same alive envs (include/b2q_es.h).  The loop over the
+// columns is unrolled to B2Q_ES_MAX_TERMS so that every cols.c[j] is a constant-bank read, never a local copy of the struct.
+template <typename T>
+__global__ void es_accumulate_terms_kernel(const T* __restrict__ reward, const uint8_t* __restrict__ done, uint8_t* __restrict__ alive,
+                                           T* __restrict__ ret, int32_t* __restrict__ len, const T* __restrict__ info, int info_dim,
+                                           TermCols cols, int ncols, T* __restrict__ term_sum, int count_col, T thresh,
+                                           int32_t* __restrict__ count, int n) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !alive[i]) return;
+  ret[i] += reward[i];
+  len[i] += 1;
+  const T* row = info + (size_t)i * info_dim;
+#pragma unroll
+  for (int j = 0; j < B2Q_ES_MAX_TERMS; j++)
+    if (j < ncols) term_sum[(size_t)j * n + i] += row[cols.c[j]];
+  if (count_col >= 0) count[i] += row[count_col] >= thresh ? 1 : 0;   // NaN >= thresh is false
+  if (done[i]) alive[i] = 0;
+}
+
 // one warp per individual: deterministic shuffle-tree sum over its `rollouts` consecutive envs
 template <typename T>
 __global__ void es_fitness_kernel(const T* __restrict__ ret, const int32_t* __restrict__ len, T* __restrict__ fitness, T* __restrict__ mean_len,
@@ -42,6 +63,29 @@ int b2q_es_accumulate(const void* reward, const uint8_t* done, uint8_t* alive, v
   cudaStream_t s = (cudaStream_t)stream;
   if (elem_size == 4) es_accumulate_kernel<float><<<(n + 255) / 256, 256, 0, s>>>((const float*)reward, done, alive, (float*)ret, len, n);
   else es_accumulate_kernel<double><<<(n + 255) / 256, 256, 0, s>>>((const double*)reward, done, alive, (double*)ret, len, n);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
+int b2q_es_accumulate_terms(const void* reward, const uint8_t* done, uint8_t* alive, void* ret, int32_t* len, const void* info, int info_dim,
+                            const int32_t* cols, int ncols, void* term_sum, int count_col, double thresh, int32_t* count, int n, int elem_size,
+                            void* stream) {
+  if (!reward || !done || !alive || !ret || !len || n < 1 || (elem_size != 4 && elem_size != 8)) return -1;
+  if (ncols < 0 || ncols > B2Q_ES_MAX_TERMS || count_col < -1) return -1;
+  if ((ncols > 0 || count_col >= 0) && (!info || info_dim < 1)) return -1;
+  if ((ncols > 0 && (!cols || !term_sum)) || (count_col >= 0 && (!count || count_col >= info_dim))) return -1;
+  TermCols tc = {};
+  for (int j = 0; j < ncols; j++) {
+    if (cols[j] < 0 || cols[j] >= info_dim) return -1;
+    tc.c[j] = cols[j];
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  int blocks = (n + 255) / 256;
+  if (elem_size == 4)
+    es_accumulate_terms_kernel<float><<<blocks, 256, 0, s>>>((const float*)reward, done, alive, (float*)ret, len, (const float*)info, info_dim, tc, ncols,
+                                                             (float*)term_sum, count_col, (float)thresh, count, n);
+  else
+    es_accumulate_terms_kernel<double><<<blocks, 256, 0, s>>>((const double*)reward, done, alive, (double*)ret, len, (const double*)info, info_dim, tc,
+                                                              ncols, (double*)term_sum, count_col, thresh, count, n);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

@@ -364,6 +364,47 @@ def gather_fitness_and_length(fl, world, rank, group=None):
     return g[:, 0, :].reshape(-1), g[:, 1, :].reshape(-1)
 
 
+SUCCESS_VELX = 0.3          # a step counts towards the success rate when info["velx"] >= 0.3 (pretrain.py:147)
+
+
+class EpisodeStats:
+    """Device buffers of one batch of episodes and the fused per-step accumulator b2q_es_accumulate_terms: return, length, the episode
+    sums of the info columns `terms` (names of _config.INFO) and the count of steps with velx >= SUCCESS_VELX, all frozen at each env's
+    first done.  The column array is built once, so step() is one launch with no host work besides the call."""
+
+    MAX_TERMS = 16          # B2Q_ES_MAX_TERMS, include/b2q_es.h
+
+    def __init__(self, lib, n, dtype, device, terms=(), count_col="velx", thresh=SUCCESS_VELX, alive=None, ret=None, length=None):
+        import torch
+        from ._config import INFO
+        if len(terms) > self.MAX_TERMS:
+            raise ValueError("at most %d terms, got %d" % (self.MAX_TERMS, len(terms)))
+        self.lib, self.n, self.terms = lib, int(n), tuple(terms)
+        self.alive = torch.ones(n, dtype=torch.uint8, device=device) if alive is None else alive
+        self.ret = torch.zeros(n, dtype=dtype, device=device) if ret is None else ret
+        self.len = torch.zeros(n, dtype=torch.int32, device=device) if length is None else length
+        self.term_sum = torch.zeros(len(self.terms), n, dtype=dtype, device=device)
+        self.count = torch.zeros(n, dtype=torch.int32, device=device)
+        self.count_col = -1 if count_col is None else INFO[count_col]
+        self.thresh = float(thresh)
+        self._cols = (C.c_int32 * self.MAX_TERMS)(*[INFO[k] for k in self.terms])
+        self._es = torch.empty((), dtype=dtype).element_size()
+
+    def zero(self):
+        self.alive.fill_(1); self.ret.zero_(); self.len.zero_(); self.term_sum.zero_(); self.count.zero_()
+
+    def step(self, reward, done, info, stream):
+        from ._config import INFO_DIM
+        rc = self.lib.b2q_es_accumulate_terms(reward.data_ptr(), done.data_ptr(), self.alive.data_ptr(), self.ret.data_ptr(), self.len.data_ptr(),
+                                              info.data_ptr(), INFO_DIM, self._cols, len(self.terms), self.term_sum.data_ptr() if self.terms else None,
+                                              self.count_col, self.thresh, self.count.data_ptr(), self.n, self._es, stream)
+        assert rc == 0, rc
+
+    def success_rate(self):
+        """[n] fraction of each episode's steps with velx >= thresh (count / length)."""
+        return self.count.to(self.ret.dtype) / self.len.to(self.ret.dtype)
+
+
 class PopulationEvaluator:
     """Evaluates this rank's shard of an ES population on its GPU and all-gathers the fitness vector."""
 
@@ -390,9 +431,14 @@ class PopulationEvaluator:
         self.es_launches = 0
         self.rows = None
 
-    def evaluate(self, etg_w, etg_b, residual_noise=None, replay=None, record=None):
+    def evaluate(self, etg_w, etg_b, residual_noise=None, replay=None, record=None, terms=None):
         """etg_w [pop,3,20], etg_b [pop,3] for the WHOLE population (identical on every rank); returns fitness[pop]
         (identical on every rank) and mean episode length[pop].
+
+        terms: a sequence of info column names (e.g. train.EVAL_TERMS).  Then the step loop uses the fused accumulator
+        (b2q_es_accumulate_terms: fitness and length bit-identical to the call without terms) and evaluate returns
+        (fitness, mean_len, term_means [len(terms), pop], success [pop]): the mean over each individual's rollouts of every term's
+        episode sum, and of the fraction of its episode's steps with velx >= SUCCESS_VELX.
 
         replay: a ReplayMemory that receives the transitions whose reward enters the fitness (run_EStrain_episode with es_rpm,
         train.py:240-241): on every step, the rows of the envs still in their first episode, of the FIRST rollout of each recorded
@@ -409,6 +455,13 @@ class PopulationEvaluator:
         self.alive.fill_(1); self.ret.zero_(); self.len.zero_()
         es = env.obs.element_size()
         stream = env._stream()
+        stats = None
+        if terms is not None:
+            terms = tuple(terms)
+            if getattr(self, "_stats", None) is None or self._stats.terms != terms:     # shares alive / ret / len with the plain path
+                self._stats = EpisodeStats(self.lib, self.n, env.dtype, env.device, terms, alive=self.alive, ret=self.ret, length=self.len)
+            stats = self._stats
+            stats.term_sum.zero_(); stats.count.zero_()
         if replay is not None:
             rec = np.ones(self.popsize, dtype=bool) if record is None else np.asarray(record, dtype=bool).reshape(self.popsize)
             rec_local = torch.as_tensor(rec[self.lo:self.hi].astype(np.uint8), device=env.device)
@@ -426,15 +479,18 @@ class PopulationEvaluator:
                 act = act + residual_noise[k]
             if replay is not None:
                 prev_obs.copy_(obs)                                 # env.step overwrites env.obs in place
-            obs, rew, done, _ = env.step(act, donef=(k + 1 > self.max_steps))
+            obs, rew, done, info = env.step(act, donef=(k + 1 > self.max_steps))
             if replay is not None:                                  # the rows whose reward b2q_es_accumulate adds below
                 torch.mul(self.alive, keep, out=mask)
                 torch.div(act, self.act_bound, out=act_out)
                 torch.sub(one, done, out=term)                      # terminal = 1 - done, train.py:229-230
                 replay.append_masked(prev_obs, act_out, rew, obs, term, mask)
-            rc = self.lib.b2q_es_accumulate(rew.data_ptr(), done.data_ptr(), self.alive.data_ptr(), self.ret.data_ptr(), self.len.data_ptr(),
-                                            self.n, es, stream)
-            assert rc == 0
+            if stats is not None:
+                stats.step(rew, done, info, stream)
+            else:
+                rc = self.lib.b2q_es_accumulate(rew.data_ptr(), done.data_ptr(), self.alive.data_ptr(), self.ret.data_ptr(), self.len.data_ptr(),
+                                                self.n, es, stream)
+                assert rc == 0
             self.es_launches += 1
         rc = self.lib.b2q_es_fitness(self.ret.data_ptr(), self.len.data_ptr(), self.fitness.data_ptr(), self.mean_len.data_ptr(),
                                      self.pop_local, self.rollouts, es, stream)
@@ -442,7 +498,15 @@ class PopulationEvaluator:
         self.es_launches += 1
         if replay is not None:
             self.rows = (self.len.reshape(self.pop_local, self.rollouts)[:, 0].long() * rec_local).sum()
-        return gather_fitness_and_length(self._fl, self.world, self.rank)
+        fitness, mean_len = gather_fitness_and_length(self._fl, self.world, self.rank)
+        if stats is None:
+            return fitness, mean_len
+        # end of the generation, off the per-step path: per-individual means over the rollouts, one all-gather of [pop_local, nt + 1]
+        nt = len(terms)
+        per_env = torch.cat([stats.term_sum, stats.success_rate()[None]], 0)
+        local = per_env.reshape(nt + 1, self.pop_local, self.rollouts).mean(2).T.contiguous()
+        full = all_gather_concat(local, self.world, self.rank).T
+        return fitness, mean_len, full[:nt], full[nt]
 
 
 DIVERGED_REWARD = -1e9      # the reward of an individual whose rollout went non-finite

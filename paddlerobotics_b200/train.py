@@ -64,7 +64,36 @@ def parser():
     p.add_argument("--render_height", type=int, default=480)
     p.add_argument("--dynamic_param", type=str, default="", help="PATH.npy: a 48-vector in [-1, 1] (dynamic_train's dynamic_param{epoch}.npy) -> "
                    "param2dynamic_dict -> every env of training, the ES phase and --eval (train.py:302-303); empty = nominal dynamics")
+    p.add_argument("--ETG_path", type=str, default="None", help="a pretrained ETG (.npz with `param`, e.g. pretrain's itr_*.npz): its 12 control-point "
+                   "offsets seed the ES solver and the first gait (train.py:281-299); a missing file keeps zero offsets.  Not with --load")
     return p
+
+
+def etg_prior(ETG_T=0.5, footheight=0.1, steplen=0.05):
+    """(layer, w0, b0, prior_points) of the default gait fit (train.py:296-299)."""
+    layer = ETG_layer(ETG_T, 0.026, 20, 0.04, np.array([-np.pi / 2, 0]), 0.2, ETG_T)
+    w0, b0, prior_points = Opt_with_points(ETG=layer, ETG_T=ETG_T, Footheight=footheight, Steplength=steplen)
+    return layer, w0, b0, prior_points
+
+
+def initial_etg(args):
+    """The ES init rule of train.py:281-287 / pretrain.py:171-177: (param [12], w, b).  If --ETG_path is an existing file, param is its `param`
+    (12 values, a 6x2 array is flattened; any other size raises ValueError naming the file) and (w, b) = Opt_with_points(prior_points + param)
+    warm-started from (w0, b0), the fit train.py:349-352 makes of the solver's best param; otherwise (zeros, w0, b0).  Nothing is written:
+    the reference's data/zero_param.npz is not created."""
+    layer, w0, b0, prior_points = etg_prior(args.ETG_T, args.footheight, args.steplen)
+    path = args.ETG_path
+    if not path or path == "None" or not os.path.isfile(path):
+        return np.zeros(12), w0, b0
+    with np.load(path) as z:
+        if "param" not in z.files:
+            raise ValueError("%s: an ETG file needs a `param` array (12 control-point offsets)" % path)
+        param = np.asarray(z["param"], dtype=np.float64)
+    if param.size != 12:
+        raise ValueError("%s: `param` must hold 12 control-point offsets, got shape %s" % (path, list(param.shape)))
+    param = param.reshape(-1).copy()
+    w, b, _ = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, w0=w0, b0=b0, points=prior_points + param.reshape(-1, 2))
+    return param, w, b
 
 
 def env_config(args):
@@ -94,6 +123,8 @@ def main(argv=None):
     w0, b0, prior_points = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, Footheight=args.footheight, Steplength=args.steplen)     # train.py:298-299
     w, b = w0, b0
     env_cfg = env_config(args)
+    if args.load and args.ETG_path not in ("", "None"):
+        p.error("--ETG_path and --load both set the ETG: --load restores (w, b, param) from the .npz next to the checkpoint")
     if args.eval:
         if not args.load:
             p.error("--eval 1 evaluates a checkpoint: it needs --load itr_*.pt")
@@ -101,7 +132,7 @@ def main(argv=None):
     # the evaluator's policy reads `learner` when it runs, so it may be built before the learner
     env, evaluator = make_envs(args, env_cfg, policy=lambda o: learner.actor.forward(o)[0][0])
     agent = MujocoAgent(49, 12, seed=args.seed)
-    ETG_best_param = np.zeros(12)                                                                                                 # ES_solver.get_best_param(), train.py:348
+    ETG_best_param, w, b = initial_etg(args)                                                                                      # ES_solver.get_best_param(), train.py:348
     if args.load:
         agent.restore(args.load)
         z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
@@ -244,45 +275,55 @@ EVAL_MAX_STEP = 600                                                         # ru
 EVAL_TERMS = ("torso", "feet", "up", "tau", "badfoot", "footcontact")       # the info terms summed per episode, train.py:202-207
 
 
+def run_evaluate_episodes(env, w, b, policy=None, act_bound=0.3, max_step=EVAL_MAX_STEP, render=None):
+    """run_evaluate_episodes (train.py:182-211): one episode per env of `env` (no auto-reset) on the ETG (w, b), at most max_step + 1
+    control steps (the reference's loop breaks after step max_step + 1; donef forces the done flag of that step).  policy(obs) -> [N,12]
+    in [-1, 1], scaled by act_bound; None = zero residual (the open-loop ETG).  Each env's return, length, EVAL_TERMS sums and velx
+    success count freeze at its first done, all in one b2q_es_accumulate_terms launch per step.  render(steps): per-step hook.
+    Returns {mean_return, mean_length, terms: {term: mean episode sum}, success_rate: mean over envs of count / length}."""
+    from . import _lib
+    from .es import EpisodeStats
+    n = env.num_envs
+    stats = EpisodeStats(_lib.load(), n, env.dtype, env.device, EVAL_TERMS)
+    stream = env._stream()
+    zero = torch.zeros(n, 12, dtype=env.dtype, device=env.device) if policy is None else None
+    obs = env.reset(w, b)
+    for steps in range(1, max_step + 2):
+        act = zero if policy is None else policy(obs) * act_bound                                        # agent.predict(obs), train.py:193
+        obs, rew, done, info = env.step(act, donef=steps > max_step)
+        if render is not None:
+            render(steps)
+        stats.step(rew, done, info, stream)
+        if not bool(stats.alive.any()):
+            break
+    return {"mean_return": float(stats.ret.double().mean()), "mean_length": float(stats.len.double().mean()),
+            "terms": {k: float(stats.term_sum[j].double().mean()) for j, k in enumerate(EVAL_TERMS)},
+            "success_rate": float(stats.success_rate().double().mean())}
+
+
+def frame_writer(env, args):
+    """--render_dir: a render hook that writes env 0's camera image of the current step to DIR/img{step}.png (train.py:196-199)."""
+    from .render import write_png
+    os.makedirs(args.render_dir, exist_ok=True)
+
+    def frame(steps):
+        rgba = env.get_camera_image(args.render_width, args.render_height, env_ids=[0])[0]
+        write_png(os.path.join(args.render_dir, "img%d.png" % steps), rgba[0].cpu().numpy())
+    return frame
+
+
 def evaluate(args, env_cfg):
     """--eval 1: one deterministic episode per env of the restored agent and ETG (w, b) on the training env's config, at most
-    EVAL_MAX_STEP + 1 control steps (the reference's loop breaks after step 601).  Each env's return, length and per-term sums are
-    frozen at its first done by the ES evaluator's accumulator (b2q_es_accumulate).  Prints and returns one JSON record."""
-    from . import _lib
-    from ._config import INFO
-    from .render import write_png
+    EVAL_MAX_STEP + 1 control steps (run_evaluate_episodes).  Prints and returns one JSON record."""
     agent = MujocoAgent(49, 12, seed=args.seed)
     agent.restore(args.load)
     z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
     w, b = z["w"], z["b"]
     n = args.eval_envs
     env = apply_dynamic_param(VecQuadrupedalEnv(n, auto_reset=False, **env_cfg), args.dynamic_param)
-    lib, dev, es, stream = _lib.load(), env.device, env.obs.element_size(), env._stream()
-    if args.render_dir:
-        os.makedirs(args.render_dir, exist_ok=True)
-    nt = len(EVAL_TERMS)
-    cols = torch.tensor([INFO[k] for k in EVAL_TERMS], device=dev)
-    alive = torch.ones(n, dtype=torch.uint8, device=dev)
-    ret, length = torch.zeros(n, dtype=env.dtype, device=dev), torch.zeros(n, dtype=torch.int32, device=dev)
-    # every term gets its own copy of `alive` per step (the accumulator clears it at done), so all sums freeze at the same step
-    t_alive, t_sum, t_len = torch.empty(nt, n, dtype=torch.uint8, device=dev), torch.zeros(nt, n, dtype=env.dtype, device=dev), torch.zeros(nt, n, dtype=torch.int32, device=dev)
-    t_val = torch.empty(nt, n, dtype=env.dtype, device=dev)
-    obs = env.reset(w, b)
-    for steps in range(1, EVAL_MAX_STEP + 2):
-        act = agent.predict_batch(obs)                                                                        # agent.predict(obs), train.py:193
-        obs, rew, done, info = env.step(act * args.act_bound, donef=steps > EVAL_MAX_STEP)
-        if args.render_dir:
-            rgba = env.get_camera_image(args.render_width, args.render_height, env_ids=[0])[0]
-            write_png(os.path.join(args.render_dir, "img%d.png" % steps), rgba[0].cpu().numpy())
-        t_val.copy_(info.index_select(1, cols).T)
-        t_alive.copy_(alive.expand(nt, n))
-        for j in range(nt):
-            assert lib.b2q_es_accumulate(t_val[j].data_ptr(), done.data_ptr(), t_alive[j].data_ptr(), t_sum[j].data_ptr(), t_len[j].data_ptr(), n, es, stream) == 0
-        assert lib.b2q_es_accumulate(rew.data_ptr(), done.data_ptr(), alive.data_ptr(), ret.data_ptr(), length.data_ptr(), n, es, stream) == 0
-        if not bool(alive.any()):
-            break
-    rec = {"eval_envs": n, "mean_return": float(ret.double().mean()), "mean_length": float(length.double().mean()),
-           "terms": {k: float(t_sum[j].double().mean()) for j, k in enumerate(EVAL_TERMS)}}
+    r = run_evaluate_episodes(env, w, b, policy=agent.predict_batch, act_bound=args.act_bound, max_step=EVAL_MAX_STEP,
+                              render=frame_writer(env, args) if args.render_dir else None)
+    rec = {"eval_envs": n, "mean_return": r["mean_return"], "mean_length": r["mean_length"], "terms": r["terms"]}
     print(json.dumps(rec), flush=True)
     env.close()
     return rec

@@ -2,7 +2,7 @@
     compute-sanitizer --tool memcheck  python scripts/sanitize.py
     compute-sanitizer --tool racecheck python scripts/sanitize.py
 """
-import os, sys
+import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from paddlerobotics_b200.env import VecQuadrupedalEnv
@@ -108,5 +108,15 @@ bcur = torch.tensor([1001 - 20], dtype=torch.int64, device="cuda")
 bcm.gather_cursor(torch.randperm(1001, device="cuda"), bcur, torch.empty(128, 46, device="cuda"), torch.empty(128, 49, device="cuda"))
 bcl = SACLearner(MujocoAgent(46, 12, seed=4), 128)
 bcl.bc_sweep(bcm, expert, torch.randperm(1001, device="cuda"), 7, seed=1, graph_steps=3)
+# fused episode statistics: a partial last block (n = 300) in both precisions with terms and a count, ncols = 0 with a NULL count, and the
+# evaluator's terms path
+from paddlerobotics_b200 import _lib
+from paddlerobotics_b200.es import EpisodeStats
+for dt in (torch.float32, torch.float64):
+    for terms, cc in ((("torso", "feet", "up", "tau", "badfoot", "footcontact"), "velx"), ((), None)):
+        st = EpisodeStats(_lib.load(), 300, dt, torch.device("cuda"), terms, count_col=cc)
+        st.step(torch.randn(300, device="cuda", dtype=dt), (torch.rand(300, device="cuda") < 0.3).to(torch.uint8), torch.randn(300, 56, device="cuda", dtype=dt),
+                C.c_void_p(torch.cuda.current_stream().cuda_stream))
+ev.evaluate(np.repeat(w[None], 4, 0), np.repeat(b[None], 4, 0), terms=("torso", "up"))
 torch.cuda.synchronize()
 print("sanitizer script done")
