@@ -32,7 +32,17 @@ struct WarpComm {
   }
   template <typename T>
   __device__ __forceinline__ T bcast(T v, int f) const { return __shfl_sync(0xffffffffu, v, f, 4); }
+#ifdef B2Q_REGION_CLOCKS
+  mutable long long t_mark = 0, cyc[RC_N] = {};   // cycles per region of this launch, in registers (every index is a constant)
+  __device__ __forceinline__ void mark(int region) const { const long long t = clock64(); cyc[region] += t - t_mark; t_mark = t; }
+#endif
 };
+
+#ifdef B2Q_REGION_CLOCKS
+// one row per warp of the step kernel, summed over launches: the RC_N region cycles, the entry-to-exit cycles and the launch count
+constexpr int RC_MAX_WARPS = 8192, RC_COLS = RC_N + 2;
+__device__ unsigned long long g_region_clocks[RC_MAX_WARPS][RC_COLS];
+#endif
 
 template <typename T>
 __device__ __forceinline__ const Model<T>& stage_model(const Model<T>* g, unsigned char* smem) {
@@ -80,6 +90,9 @@ __device__ __forceinline__ void emit_obs_block(const Model<T>& md, const T* stag
 template <typename T, int FEAT>
 __global__ void __launch_bounds__(128) b2q_step_kernel(Cfg<T> cf, const Model<T>* __restrict__ gm, Buffers<T> B, const T* __restrict__ action, int donef,
                                                        int auto_reset, T* __restrict__ obs, T* __restrict__ reward, uint8_t* __restrict__ done, T* __restrict__ info) {
+#ifdef B2Q_REGION_CLOCKS
+  const long long t_entry = clock64();
+#endif
   extern __shared__ __align__(32) unsigned char smem[];
   const Model<T>& md = stage_model(gm, smem);
   // the CTA's observation rows are contiguous in [N][OBS_DIM]: stage them in shared memory and store the block with
@@ -99,11 +112,24 @@ __global__ void __launch_bounds__(128) b2q_step_kernel(Cfg<T> cf, const Model<T>
   // the info rows (56 floats per env, produced in 3-float pieces) are staged the same way: one coalesced block per CTA, so that `info`
   // too may be pinned HOST memory (train.py:150-157 reads info every step)
   T* istage = istage0;
+#ifdef B2Q_REGION_CLOCKS
+  cm.t_mark = t_entry;
+#endif
   step_lane<T, FEAT>(cm, cf, md, B, env, valid, action, donef, auto_reset, stage + (ptrdiff_t)(srow - env) * OBS_DIM, reward, done, istage, env0, env0);
   __syncthreads();
   const int rows = min(per_cta, B.N - env0);
   emit_obs_block(md, stage, obs, env0, rows);
   copy_block(info + (size_t)env0 * INFO_DIM, istage, rows * INFO_DIM);
+#ifdef B2Q_REGION_CLOCKS
+  B2Q_MARK(cm, RC_EPILOGUE);
+  const int warp = (int)(gid >> 5);
+  if ((threadIdx.x & 31) == 0 && warp < RC_MAX_WARPS) {   // launches on one stream run one after another: plain read-modify-write
+#pragma unroll
+    for (int r = 0; r < RC_N; r++) g_region_clocks[warp][r] += (unsigned long long)cm.cyc[r];
+    g_region_clocks[warp][RC_N] += (unsigned long long)(cm.t_mark - t_entry);
+    g_region_clocks[warp][RC_N + 1] += 1;
+  }
+#endif
 }
 
 template <typename T, int FEAT>
@@ -492,5 +518,24 @@ int b2q_render(B2QHandle h, const void* state, const int32_t* env_ids, int V, co
                float* depth, int32_t* seg, void* stream) {
   return h ? h->impl->render(state, env_ids, V, view, proj, width, height, rgba, depth, seg, (cudaStream_t)stream) : B2Q_EINVAL;
 }
+
+#ifdef B2Q_REGION_CLOCKS
+// Debug ABI of the region-clock build only (not in include/b2q.h, absent from the product library): waits for the device, copies the
+// first n_warps rows of the step kernel's region clocks to `out` ([n_warps][8] u64: the RC_* regions of b2q_sim.cuh, entry-to-exit
+// cycles, launches; may be NULL) and zeroes every row when `clear` is set.
+int b2q_region_clocks(int device, uint64_t* out, int n_warps, int clear) {
+  static_assert(RC_COLS == 8, "the row layout documented above");
+  if (n_warps < 0 || n_warps > RC_MAX_WARPS) return B2Q_EINVAL;
+  if (cudaSetDevice(device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) return B2Q_ECUDA;
+  const size_t bytes = (size_t)n_warps * RC_COLS * sizeof(unsigned long long);
+  if (out && bytes && cudaMemcpyFromSymbol(out, g_region_clocks, bytes) != cudaSuccess) return B2Q_ECUDA;
+  if (clear) {
+    void* p = nullptr;
+    if (cudaGetSymbolAddress(&p, g_region_clocks) != cudaSuccess || cudaMemset(p, 0, sizeof(g_region_clocks)) != cudaSuccess) return B2Q_ECUDA;
+    if (cudaDeviceSynchronize() != cudaSuccess) return B2Q_ECUDA;
+  }
+  return B2Q_OK;
+}
+#endif
 
 }  // extern "C"

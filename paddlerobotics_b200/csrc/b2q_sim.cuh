@@ -99,6 +99,16 @@ struct LaneState {
 
 template <typename T> B2Q_HD void sincos_t(T a, T& s, T& c) { m_sincos(a, s, c); }
 
+// Region clocks of the step kernel, compiled in only with -DB2Q_REGION_CLOCKS (scripts/step_regions.py builds that library apart from
+// the product one).  A mark reads clock64(), charges the cycles since the previous mark to the region that ends there and opens the next.
+// The product build expands every mark to nothing.
+enum { RC_PROLOGUE, RC_PRE_SWEEP, RC_SWEEP, RC_POST_SWEEP, RC_BETWEEN, RC_EPILOGUE, RC_N };
+#if defined(B2Q_REGION_CLOCKS) && defined(__CUDA_ARCH__)
+#define B2Q_MARK(cm, region) (cm).mark(region)
+#else
+#define B2Q_MARK(cm, region) ((void)0)
+#endif
+
 // ---------------------------------------------------------------------------------------------------------------
 // terrain: plane or bilinear height field
 template <typename T>
@@ -269,6 +279,7 @@ B2Q_HD void solve_rows36(const Comm& cm, const Cfg<T>& cf, T mu, const T (*Y)[6]
 template <typename T, int FEAT, class Comm>
 B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const LaneParam<T>& pr, LaneState<T>& s,
                     const T* target, T* tau_out, V3<T> fext = V3<T>{0, 0, 0}, const T* hyb = nullptr /*HYBRID: kp[3] | qd*[3] | kd[3] | tau_ff[3]*/) {
+  B2Q_MARK(cm, RC_BETWEEN);
   const int k = cm.leg();
   const LegModel<T>& lm = md.leg[k];
   const T dt = cf.dt, idt = cf.idt;
@@ -665,14 +676,20 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     // (measured: alternating between two areas instead costs 10 % — more shared memory per CTA and parity-dependent addressing)
     cm.sync();
   }
+  B2Q_MARK(cm, RC_PRE_SWEEP);
   // --- projected Gauss-Seidel, Bullet row order: normals of feet 0..3, then (t1,t2) of feet 0..3.
   //     Row update = clamp -> delta -> 11 independent scalar FFMAs (W'_rr = 0: the row's own candidate is unchanged).
+  //     A sweep in which no lambda changes (every dl = 0) leaves g unchanged too, so every later sweep would repeat it exactly: the
+  //     lane leaves the loop there and the result is the one all cf.iters sweeps give.  `moved` sums |dl| (zero only if every dl is,
+  //     NaN keeps it nonzero); the warp leaves once all 8 robots are at such a fixed point (measured on H100: sweep time -22 %).
   for (int it = 0; it < cf.iters; it++) {
+    T moved = T(0);
 #pragma unroll
     for (int f = 0; f < 4; f++) {
       const int r = 3 * f;
       T ln = m_max(g[r], T(0));
       T dl = lam[r] - ln; lam[r] = ln;          // dl = -(delta lambda)
+      moved += m_abs(dl);
 #pragma unroll
       for (int i = 0; i < 12; i++)
         if (i != r) g[i] = m_fma(Wc[r][i], dl, g[i]);
@@ -685,12 +702,15 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
         T lim = pr.mu * lam[3 * f];
         T ln = m_min(m_max(g[r], -lim), lim);
         T dl = lam[r] - ln; lam[r] = ln;
+        moved += m_abs(dl);
 #pragma unroll
         for (int i = 0; i < 12; i++)
           if (i != r) g[i] = m_fma(Wc[r][i], dl, g[i]);
       }
     }
+    if (moved == T(0)) break;
   }
+  B2Q_MARK(cm, RC_SWEEP);
 #pragma unroll
   for (int f = 0; f < 4; f++) if (f == k) { lk[0] = lam[3 * f]; lk[1] = lam[3 * f + 1]; lk[2] = lam[3 * f + 2]; }   // own impulses (no dynamic register indexing)
   }
@@ -731,6 +751,7 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     T nn = m_rsqrt(ox * ox + oy * oy + oz * oz + ow * ow);
     s.qx = ox * nn; s.qy = oy * nn; s.qz = oz * nn; s.qw = ow * nn;
   }
+  B2Q_MARK(cm, RC_POST_SWEEP);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -940,6 +961,7 @@ B2Q_HD void step_lane(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, cons
   int ib = ((R - 2 - n_lag) % R + R) % R, mb = (n_lag + 1 - (R - 1 - ib)) / R;
   const int slot = step % B.Dm;
   T tau[3] = {0, 0, 0};
+  B2Q_MARK(cm, RC_PROLOGUE);
 #pragma unroll 1
   for (int i = 0; i < R; i++) {  // Minitaur.Step, minitaur.py:248-260
     T proc[3];
@@ -955,6 +977,7 @@ B2Q_HD void step_lane(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, cons
     if (valid && i == ia) ring_write(B, slot, 0, k, env, s.q, s.qd, tau);
     if (valid && i == ib) ring_write(B, slot, 1, k, env, s.q, s.qd, tau);
   }
+  B2Q_MARK(cm, RC_BETWEEN);
 #pragma unroll
   for (int j = 0; j < 3; j++) last_action[j] = target[j];
   has_last = 1;
