@@ -73,6 +73,9 @@ SYMBOLS = {
     "b2q_bc_gather_cursor": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     # camera images — include/b2q_render.h
     "b2q_render": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    # deployment rehearsal — include/b2q_deploy.h
+    "b2q_deploy_obs": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp]),
+    "b2q_deploy_act": (_i, [_vp, _vp, C.c_double, _vp, _i, _vp, _vp, _i, _vp]),
 }
 
 

@@ -10,6 +10,7 @@
 #include <new>
 #include <string>
 #include "b2q_host_common.h"
+#include "b2q_env_view.h"
 #include "b2q_render_internal.h"
 #include "../../include/b2q_render.h"
 
@@ -222,6 +223,7 @@ struct EnvBase {
   virtual void set_max_steps(int m) = 0;
   virtual int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
                      int32_t* seg, cudaStream_t s) = 0;
+  virtual void view(EnvView* v) const = 0;
 };
 
 #define CK(call)                                                                      \
@@ -438,6 +440,9 @@ struct EnvT : EnvBase {
     return B2Q_OK;
   }
   void set_max_steps(int m) override { cfg.max_episode_steps = m; kc.max_steps = m; }   // kc goes to the step kernel by value
+  void view(EnvView* v) const override {
+    v->N = B.N; v->obs_dim = obs_dim; v->elem_size = (int)sizeof(T); v->device = cfg.device; v->step_count = B.step_count; v->model = d_model;
+  }
   int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
              int32_t* seg, cudaStream_t s) override {
     if (!state || !env_ids || !view || !proj) { err = "b2q_render: null state, env_ids, view or proj"; return B2Q_EINVAL; }
@@ -460,6 +465,15 @@ struct EnvT : EnvBase {
 }  // namespace
 
 struct B2QEnv { EnvBase* impl; };
+
+namespace b2q {
+int env_view(B2QHandle h, EnvView* v) {
+  if (!h || !v) return B2Q_EINVAL;
+  h->impl->view(v);
+  return B2Q_OK;
+}
+void env_set_error(B2QHandle h, const char* msg) { if (h) h->impl->err = msg; }
+}  // namespace b2q
 
 extern "C" {
 

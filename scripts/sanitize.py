@@ -118,5 +118,20 @@ for dt in (torch.float32, torch.float64):
         st.step(torch.randn(300, device="cuda", dtype=dt), (torch.rand(300, device="cuda") < 0.3).to(torch.uint8), torch.randn(300, 56, device="cuda", dtype=dt),
                 C.c_void_p(torch.cuda.current_stream().cuda_stream))
 ev.evaluate(np.repeat(w[None], 4, 0), np.repeat(b[None], 4, 0), terms=("torso", "up"))
+# deployment rehearsal: both kernels in both precisions on a partial last block (13 envs x 12 columns), counters past the table (NaN rows),
+# a record shorter than the rollout, and no ETG block
+from paddlerobotics_b200 import deploy
+for prec in ("f32", "f64"):
+    for kw in (dict(), dict(sensor_etg=0, sensor_dis=0)):
+        env = VecQuadrupedalEnv(13, precision=prec, etg_enabled=0, **kw)
+        tab = torch.randn(4, 12, device="cuda", dtype=env.dtype)
+        rec_o, rec_a = torch.empty(3, env.observation_dim, device="cuda", dtype=env.dtype), torch.empty(3, 12, device="cuda", dtype=env.dtype)
+        act = torch.empty(13, 12, device="cuda", dtype=env.dtype)
+        obs = env.reset()
+        for _ in range(6):
+            deploy.deploy_obs(env, tab, 4, obs, rec_o)
+            deploy.deploy_act(env, torch.rand(13, 12, device="cuda") * 2 - 1, 0.3, tab, 4, act, rec_a)
+            obs = env.step(act)[0]
+        torch.cuda.synchronize(); env.close()
 torch.cuda.synchronize()
 print("sanitizer script done")
