@@ -17,6 +17,9 @@ namespace b2q {
 // ---- scalar math wrappers (precise variants: no fast-math intrinsics, parity with the f64 oracle matters)
 B2Q_HD float m_sqrt(float x) { return sqrtf(x); }
 B2Q_HD double m_sqrt(double x) { return sqrt(x); }
+// m_rsqrt(float): rsqrtf on the device, <= 1.52 ulp over every positive normal float (measured exhaustively on H100, tests/gpu_probe); the
+// host build's 1.0f / sqrtf(x) rounds twice, <= 1.48 ulp, and differs from the device in about a third of the inputs.  Callers: chol6's
+// pivots, terrain normals, contact tangents and the quaternion renormalisation, all positive and normal.
 #if defined(__CUDA_ARCH__)
 B2Q_HD float m_rsqrt(float x) { return rsqrtf(x); }
 #else
@@ -76,7 +79,11 @@ template <typename T> B2Q_HD void philox_normal4(uint64_t seed, uint32_t c0, uin
   n[0] = ra * m_cos(two_pi * u1); n[1] = ra * m_sin(two_pi * u1); n[2] = rb * m_cos(two_pi * u3); n[3] = rb * m_sin(two_pi * u3);
 }
 
-// reciprocal: one MUFU.RCP + one Newton step on the GPU (<= 1 ulp, no slow path / branch); exact division elsewhere
+// reciprocal: one MUFU.RCP + one Newton step on the GPU (no slow path / branch); exact division elsewhere.  Measured exhaustively on H100
+// (tests/gpu_probe): for every normal x with |x| <= 2^126 the device result is the correctly rounded 1/x, the host's.  The edges follow
+// from rcp.approx.ftz: x = +-0, +-inf and subnormal x give NaN (the Newton step computes 0 * inf or inf - inf), |x| > 2^126 gives a
+// signed zero instead of the subnormal 1/x.  No caller reaches them: det of the 3x3 joint-space block and W_ii of an active contact
+// row are positive and far inside the normal range, and sh / th runs only for th >= 1e-4.
 #if defined(__CUDA_ARCH__)
 B2Q_HD float m_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return fmaf(r, fmaf(-x, r, 1.0f), r); }
 #else
@@ -85,8 +92,11 @@ B2Q_HD float m_rcp(float x) { return 1.0f / x; }
 B2Q_HD double m_rcp(double x) { return 1.0 / x; }
 
 // sin and cos together for |a| up to a few turns (joint angles, Euler-step rotation angles): Cody-Waite reduction by
-// pi/2 (3 constants) + the classic degree-7/8 minimax kernels on [-pi/4, pi/4]; ~1 ulp, branch-free, ~30 instructions
+// pi/2 (3 constants) + the classic degree-7/8 minimax kernels on [-pi/4, pi/4]; branch-free, ~30 instructions
 // (libm's sinf/cosf carry a Payne-Hanek slow path that costs >2000 instructions of code in this kernel).
+// Measured over all 2.2e9 floats in [-8 pi, 8 pi] on H100 (tests/gpu_probe): <= 1.50 ulp for sin, <= 1.49 ulp for cos, the host
+// build bit-identical.  Sampled up to |a| = 2^20 the outputs stay finite with s^2 + c^2 within 1.5 eps of 1; NaN and +-inf give NaN.
+// The callers need |a| < 8 pi: leg_kin's q1, q2 and q1 + q2 (|q1 + q2| < 6.9 over the URDF ranges) and the Euler step's |w| dt / 2.
 B2Q_HD void m_sincos(float a, float& s, float& c) {
   float q = rintf(a * 0.636619772367581343f);            // nearest multiple of pi/2
   int n = (int)q;

@@ -12,6 +12,7 @@
 #include <thread>
 #include <vector>
 #include "../../paddlerobotics_b200/csrc/b2q_host_common.h"
+#include "../gpu_probe/prim.h"
 
 using namespace b2q;
 
@@ -183,5 +184,47 @@ int emu_set_state(void* hv, const void* in) {
   if (h->prec) { auto* e = (Emu<double>*)h->p; for (int i = 0; i < e->B.N; i++) set_state_env<double>(e->state.data(), (const double*)in, e->B.N, i); }
   else { auto* e = (Emu<float>*)h->p; for (int i = 0; i < e->B.N; i++) set_state_env<float>(e->state.data(), (const float*)in, e->B.N, i); }
   return 0;
+}
+
+// ---- the scalar primitives through their host branches, one element at a time (tests/gpu_probe/prim.h; the probe runs the device ones)
+void emu_sincos_f(int n, const float* a, float* s, float* c) { for (int i = 0; i < n; i++) b2q_prim::sincos_f(a[i], s + i, c + i); }
+void emu_unary_f(int which, int n, const float* x, float* y) { for (int i = 0; i < n; i++) y[i] = which == 0 ? b2q_prim::rcp_f(x[i]) : b2q_prim::rsqrt_f(x[i]); }
+void emu_philox4(int n, const uint64_t* seed, const uint32_t* ctr, uint32_t* out) {
+  for (int i = 0; i < n; i++) philox4(seed[i], ctr[3 * i], ctr[3 * i + 1], ctr[3 * i + 2], out + 4 * i);
+}
+void emu_philox_normal4(int prec, int n, const uint64_t* seed, const uint32_t* ctr, void* out) {
+  for (int i = 0; i < n; i++) {
+    if (prec) philox_normal4<double>(seed[i], ctr[3 * i], ctr[3 * i + 1], ctr[3 * i + 2], (double*)out + 4 * i);
+    else philox_normal4<float>(seed[i], ctr[3 * i], ctr[3 * i + 1], ctr[3 * i + 2], (float*)out + 4 * i);
+  }
+}
+void emu_leg(int prec, int n, int inverse, const int* leg, const void* in, void* out) {
+  if (prec) {
+    Model<double> md = b2q_prim::default_model<double>(); const double* x = (const double*)in; double* y = (double*)out;
+    for (int i = 0; i < n; i++) if (leg[i] >= 0 && leg[i] < 4) { if (inverse) b2q_prim::leg_inv(md, leg[i], x + 3 * i, y + 3 * i); else b2q_prim::leg_fk(md, leg[i], x + 3 * i, y + 3 * i); }
+  } else {
+    Model<float> md = b2q_prim::default_model<float>(); const float* x = (const float*)in; float* y = (float*)out;
+    for (int i = 0; i < n; i++) if (leg[i] >= 0 && leg[i] < 4) { if (inverse) b2q_prim::leg_inv(md, leg[i], x + 3 * i, y + 3 * i); else b2q_prim::leg_fk(md, leg[i], x + 3 * i, y + 3 * i); }
+  }
+}
+void emu_rpy(int prec, int n, const void* q, void* out) {
+  for (int i = 0; i < n; i++) {
+    if (prec) b2q_prim::rpy((const double*)q + 4 * i, (double*)out + 3 * i); else b2q_prim::rpy((const float*)q + 4 * i, (float*)out + 3 * i);
+  }
+}
+void emu_terrain(int prec, int nx, int ny, double x0, double y0, double cell, const double* hf, int n, const void* xy, void* out) {
+  if (prec) {
+    std::vector<double> h(hf, hf + (size_t)nx * ny); Cfg<double> cf = b2q_prim::hf_cfg<double>(nx, ny, x0, y0, cell, h.data());
+    for (int i = 0; i < n; i++) b2q_prim::terrain(cf, ((const double*)xy)[2 * i], ((const double*)xy)[2 * i + 1], (double*)out + 4 * i);
+  } else {
+    std::vector<float> h(hf, hf + (size_t)nx * ny); Cfg<float> cf = b2q_prim::hf_cfg<float>(nx, ny, x0, y0, cell, h.data());
+    for (int i = 0; i < n; i++) b2q_prim::terrain(cf, ((const float*)xy)[2 * i], ((const float*)xy)[2 * i + 1], (float*)out + 4 * i);
+  }
+}
+void emu_solve(int prec, int n, const void* S, const void* b, void* x) {
+  for (int i = 0; i < n; i++) {
+    if (prec) b2q_prim::spd_solve((const double*)S + 21 * i, (const double*)b + 6 * i, (double*)x + 6 * i);
+    else b2q_prim::spd_solve((const float*)S + 21 * i, (const float*)b + 6 * i, (float*)x + 6 * i);
+  }
 }
 }

@@ -101,3 +101,66 @@ class EmuEnv:
         if self.h:
             lib().emu_destroy(self.h)
             self.h = None
+
+
+# ---- the step kernel's scalar primitives through their host branches (same call surface as tests/gpu_probe/probe.py)
+def _p(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+
+def _dt(prec):
+    return np.float64 if prec else np.float32
+
+
+def sincos(a):
+    a = np.ascontiguousarray(a, dtype=np.float32); s, c = np.zeros_like(a), np.zeros_like(a)
+    lib().emu_sincos_f(a.size, _p(a), _p(s), _p(c))
+    return s, c
+
+
+def unary(which, x):
+    """m_rcp (0) or m_rsqrt (1) of a float32 array."""
+    x = np.ascontiguousarray(x, dtype=np.float32); y = np.zeros_like(x)
+    lib().emu_unary_f(which, x.size, _p(x), _p(y))
+    return y
+
+
+def philox4(seeds, ctr):
+    seeds = np.ascontiguousarray(seeds, dtype=np.uint64); ctr = np.ascontiguousarray(ctr, dtype=np.uint32).reshape(-1, 3)
+    out = np.zeros((seeds.size, 4), dtype=np.uint32)
+    lib().emu_philox4(seeds.size, _p(seeds), _p(ctr), _p(out))
+    return out
+
+
+def philox_normal4(prec, seeds, ctr):
+    seeds = np.ascontiguousarray(seeds, dtype=np.uint64); ctr = np.ascontiguousarray(ctr, dtype=np.uint32).reshape(-1, 3)
+    out = np.zeros((seeds.size, 4), dtype=_dt(prec))
+    lib().emu_philox_normal4(prec, seeds.size, _p(seeds), _p(ctr), _p(out))
+    return out
+
+
+def leg(prec, legs, x, inverse):
+    legs = np.ascontiguousarray(legs, dtype=np.int32); x = np.ascontiguousarray(x, dtype=_dt(prec)).reshape(-1, 3)
+    out = np.zeros_like(x)
+    lib().emu_leg(prec, legs.size, int(inverse), _p(legs), _p(x), _p(out))
+    return out
+
+
+def rpy(prec, q):
+    q = np.ascontiguousarray(q, dtype=_dt(prec)).reshape(-1, 4); out = np.zeros((q.shape[0], 3), dtype=q.dtype)
+    lib().emu_rpy(prec, q.shape[0], _p(q), _p(out))
+    return out
+
+
+def terrain(prec, hf, x0, y0, cell, xy):
+    hf = np.ascontiguousarray(hf, dtype=np.float64); xy = np.ascontiguousarray(xy, dtype=_dt(prec)).reshape(-1, 2)
+    out = np.zeros((xy.shape[0], 4), dtype=xy.dtype)
+    lib().emu_terrain(prec, hf.shape[1], hf.shape[0], C.c_double(x0), C.c_double(y0), C.c_double(cell), _p(hf), xy.shape[0], _p(xy), _p(out))
+    return out
+
+
+def solve(prec, S21, b):
+    S21 = np.ascontiguousarray(S21, dtype=_dt(prec)).reshape(-1, 21); b = np.ascontiguousarray(b, dtype=_dt(prec)).reshape(-1, 6)
+    x = np.zeros_like(b)
+    lib().emu_solve(prec, b.shape[0], _p(S21), _p(b), _p(x))
+    return x
