@@ -27,6 +27,23 @@ int b2q_es_accumulate(const void* reward, const uint8_t* done, uint8_t* alive, v
 int b2q_es_accumulate_terms(const void* reward, const uint8_t* done, uint8_t* alive, void* ret, int32_t* len, const void* info, int info_dim,
                             const int32_t* cols, int ncols, void* term_sum, int count_col, double thresh, int32_t* count, int n, int elem_size,
                             void* stream);
+/* The per-episode statistics of auto-reset TRAINING envs (train.py:150-157,175,359-366 run_train_episode) in ONE launch per control step,
+ * with no host-dependent argument, so the call can be captured in a training iteration's CUDA graph.  Unlike b2q_es_accumulate_terms an
+ * episode ends at EVERY done and the next one starts at the following step.  All sums are double, whatever elem_size is.
+ *   run [3 + ncols][n] (row r of env i at run[r*n + i]): the running episode: 0 return, 1 length, 2 count, 3 + j term j's sum
+ *   win [5 + 2*ncols][n]: the window of closed episodes: 0 episodes, 1 non-finite episodes, 2 Σ return, 3 Σ length, 4 Σ count / length,
+ *                         5 + j Σ term j, 5 + ncols + j Σ term j / length
+ * For every env i:
+ *   run_ret += reward[i]; run_len += 1; run_term[j] += info[i*info_dim + cols[j]]          for j < ncols
+ *   run_cnt += (double)info[i*info_dim + count_col] >= thresh                               (when count_col >= 0; NaN does not count)
+ *   if done[i]: if run_ret and every run_term[j] are finite, win_episodes += 1 and the episode's sums are added to rows 2..; otherwise
+ *               only win_nonfinite += 1.  Then the running row is zeroed.
+ * Zero run and win before the first call; zero run to drop the running episodes (after a hard reset), win after reading it.
+ * cols: HOST array of ncols (0..B2Q_ES_MAX_TERMS) info columns, passed by value.  count_col = -1: no count (row 4 stays 0).
+ * Returns -1 (nothing written) for a NULL required pointer, ncols out of range, a column outside [0, info_dim) or a bad elem_size;
+ * -2 on a launch error. */
+int b2q_train_episode_stats(const void* reward, const uint8_t* done, const void* info, int info_dim, const int32_t* cols, int ncols, int count_col,
+                            double thresh, double* run, double* win, int n, int elem_size, void* stream);
 /* fitness[i] = mean over the individual's rollouts of ret; mean_len (may be NULL) likewise for episode lengths. */
 int b2q_es_fitness(const void* ret, const int32_t* len, void* fitness, void* mean_len, int pop, int rollouts, int elem_size, void* stream);
 /* Batched ETG fit (SURVEY §8f-1): for each individual i, points = prior_points + solutions[i].reshape(6,2) and

@@ -59,6 +59,7 @@ SYMBOLS = {
     # ES population fitness — include/b2q_es.h
     "b2q_es_accumulate": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "b2q_es_accumulate_terms": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, C.c_double, _vp, _i, _i, _vp]),
+    "b2q_train_episode_stats": (_i, [_vp, _vp, _vp, _i, _vp, _i, _i, C.c_double, _vp, _vp, _i, _i, _vp]),
     "b2q_es_fitness": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "b2q_dyn_accumulate": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp]),
     "b2q_dyn_finish": (_i, [_vp, _i, _vp, _i, _i, _vp]),

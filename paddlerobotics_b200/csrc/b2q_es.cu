@@ -41,6 +41,50 @@ __global__ void es_accumulate_terms_kernel(const T* __restrict__ reward, const u
   if (done[i]) alive[i] = 0;
 }
 
+// Per-episode statistics of auto-reset training envs (include/b2q_es.h, b2q_train_episode_stats).  Sums in double whatever T is; an
+// episode is closed at every done.  Term sums stay in registers between the running update and the fold, so each row is read once.
+template <typename T>
+__global__ void train_episode_stats_kernel(const T* __restrict__ reward, const uint8_t* __restrict__ done, const T* __restrict__ info, int info_dim,
+                                           TermCols cols, int ncols, int count_col, double thresh, double* __restrict__ run,
+                                           double* __restrict__ win, int n) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const size_t N = (size_t)n;
+  const T* row = info + (size_t)i * info_dim;
+  double ret = run[i] + (double)reward[i];
+  double len = run[N + i] + 1.0;
+  double cnt = run[2 * N + i];
+  if (count_col >= 0) cnt += (double)row[count_col] >= thresh ? 1.0 : 0.0;   // NaN >= thresh is false
+  bool ok = isfinite(ret);
+  double term[B2Q_ES_MAX_TERMS];
+#pragma unroll
+  for (int j = 0; j < B2Q_ES_MAX_TERMS; j++)
+    if (j < ncols) { term[j] = run[(3 + j) * N + i] + (double)row[cols.c[j]]; ok = ok && isfinite(term[j]); }
+  if (!done[i]) {
+    run[i] = ret; run[N + i] = len; run[2 * N + i] = cnt;
+#pragma unroll
+    for (int j = 0; j < B2Q_ES_MAX_TERMS; j++)
+      if (j < ncols) run[(3 + j) * N + i] = term[j];
+    return;
+  }
+  // the episode ends: fold it into the window (or only count it, when a sum is not finite) and start the next one from zero
+  if (ok) {
+    win[i] += 1.0;
+    win[2 * N + i] += ret;
+    win[3 * N + i] += len;
+    if (count_col >= 0) win[4 * N + i] += cnt / len;
+#pragma unroll
+    for (int j = 0; j < B2Q_ES_MAX_TERMS; j++)
+      if (j < ncols) { win[(5 + j) * N + i] += term[j]; win[(5 + ncols + j) * N + i] += term[j] / len; }
+  } else {
+    win[N + i] += 1.0;
+  }
+  run[i] = 0.0; run[N + i] = 0.0; run[2 * N + i] = 0.0;
+#pragma unroll
+  for (int j = 0; j < B2Q_ES_MAX_TERMS; j++)
+    if (j < ncols) run[(3 + j) * N + i] = 0.0;
+}
+
 // one warp per individual: deterministic shuffle-tree sum over its `rollouts` consecutive envs
 template <typename T>
 __global__ void es_fitness_kernel(const T* __restrict__ ret, const int32_t* __restrict__ len, T* __restrict__ fitness, T* __restrict__ mean_len,
@@ -86,6 +130,28 @@ int b2q_es_accumulate_terms(const void* reward, const uint8_t* done, uint8_t* al
   else
     es_accumulate_terms_kernel<double><<<blocks, 256, 0, s>>>((const double*)reward, done, alive, (double*)ret, len, (const double*)info, info_dim, tc,
                                                               ncols, (double*)term_sum, count_col, thresh, count, n);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
+int b2q_train_episode_stats(const void* reward, const uint8_t* done, const void* info, int info_dim, const int32_t* cols, int ncols, int count_col,
+                            double thresh, double* run, double* win, int n, int elem_size, void* stream) {
+  if (!reward || !done || !run || !win || n < 1 || (elem_size != 4 && elem_size != 8)) return -1;
+  if (ncols < 0 || ncols > B2Q_ES_MAX_TERMS || count_col < -1) return -1;
+  if ((ncols > 0 || count_col >= 0) && (!info || info_dim < 1)) return -1;
+  if ((ncols > 0 && !cols) || count_col >= info_dim) return -1;
+  TermCols tc = {};
+  for (int j = 0; j < ncols; j++) {
+    if (cols[j] < 0 || cols[j] >= info_dim) return -1;
+    tc.c[j] = cols[j];
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  int blocks = (n + 255) / 256;
+  if (elem_size == 4)
+    train_episode_stats_kernel<float><<<blocks, 256, 0, s>>>((const float*)reward, done, (const float*)info, info_dim, tc, ncols, count_col, thresh,
+                                                             run, win, n);
+  else
+    train_episode_stats_kernel<double><<<blocks, 256, 0, s>>>((const double*)reward, done, (const double*)info, info_dim, tc, ncols, count_col, thresh,
+                                                              run, win, n);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

@@ -405,6 +405,47 @@ class EpisodeStats:
         return self.count.to(self.ret.dtype) / self.len.to(self.ret.dtype)
 
 
+class TrainEpisodeStats:
+    """Per-episode statistics of auto-reset training envs (b2q_train_episode_stats, include/b2q_es.h): one launch per control step closes an
+    episode at every done and folds it into per-env window sums, in double.  `run` [3 + nt, n] holds the running episodes and `win`
+    [5 + 2 nt, n] the window; both keep their storage for the object's lifetime, so step() can be captured in a CUDA graph."""
+
+    def __init__(self, lib, n, device, terms=(), count_col="velx", thresh=SUCCESS_VELX):
+        import torch
+        from ._config import INFO
+        if len(terms) > EpisodeStats.MAX_TERMS:
+            raise ValueError("at most %d terms, got %d" % (EpisodeStats.MAX_TERMS, len(terms)))
+        self.lib, self.n, self.terms = lib, int(n), tuple(terms)
+        nt = len(self.terms)
+        self.run = torch.zeros(3 + nt, self.n, dtype=torch.float64, device=device)
+        self.win = torch.zeros(5 + 2 * nt, self.n, dtype=torch.float64, device=device)
+        self.count_col = -1 if count_col is None else INFO[count_col]
+        self.thresh = float(thresh)
+        self._cols = (C.c_int32 * EpisodeStats.MAX_TERMS)(*[INFO[k] for k in self.terms])
+
+    def step(self, reward, done, info, stream):
+        from ._config import INFO_DIM
+        rc = self.lib.b2q_train_episode_stats(reward.data_ptr(), done.data_ptr(), info.data_ptr(), INFO_DIM, self._cols, len(self.terms), self.count_col,
+                                              self.thresh, self.run.data_ptr(), self.win.data_ptr(), self.n, reward.element_size(), stream)
+        assert rc == 0, rc
+
+    def restart(self):
+        """Drops the running episodes (after a hard env.reset): the next step starts a new episode in every env."""
+        self.run.zero_()
+
+    def take(self):
+        """The window's means over its finite episodes, then an empty window.  {episodes, nonfinite_episodes, return, length, terms: {term:
+        mean episode sum}, mean_terms: {term: mean of sum / length}, success_rate}; the means are None when no finite episode closed."""
+        nt = len(self.terms)
+        s = self.win.sum(1).tolist()
+        self.win.zero_()
+        k = s[0]
+        m = (lambda x: x / k) if k > 0 else (lambda x: None)
+        return {"episodes": int(k), "nonfinite_episodes": int(s[1]), "return": m(s[2]), "length": m(s[3]),
+                "success_rate": m(s[4]) if self.count_col >= 0 else None,
+                "terms": {t: m(s[5 + j]) for j, t in enumerate(self.terms)}, "mean_terms": {t: m(s[5 + nt + j]) for j, t in enumerate(self.terms)}}
+
+
 class PopulationEvaluator:
     """Evaluates this rank's shard of an ES population on its GPU and all-gathers the fitness vector."""
 

@@ -1,9 +1,14 @@
 """ETG-RL training loop on the GPU engine — the batched counterpart of ETGRL/train.py:252-449 (same phases, same flag names
 where they exist): SAC episodes with one learner step per control step (train.py:163-169) over N parallel envs, and every
 `ES_EVERY_STEPS` env steps an ES phase of `ES_TRAIN_STEPS` generations over the ETG control points (train.py:392-437).
-Everything per-step stays on the device: obs -> fused MLP (wgmma) -> step kernel -> device replay -> SAC learn (CUDA graph).
+Everything per-step stays on the device: obs -> fused MLP (wgmma) -> step kernel -> device replay -> SAC learn (CUDA graph), and the
+per-episode statistics of train.py:150-157 (b2q_train_episode_stats), which every log record reads.  Every --eval_every_steps the block of
+train.py:370-390 runs: a deterministic evaluation on --train_eval_envs envs, the e_step growth of --e_step_growth, the checkpoint of --outdir.
+The reference's flags are honoured or refused before any device work (check_supported); --epsilon, --gamma, --random, --timesteps and
+--timeinterval are accepted and ignored, as in the reference.
 
     python -m paddlerobotics_b200.train --num_envs 4096 --max_steps 2000000 --ES 1
+    python -m paddlerobotics_b200.train --train_eval_envs 16 --e_step_growth 50 --outdir train_log
 """
 import argparse
 import json
@@ -13,9 +18,10 @@ import time
 import numpy as np
 import torch
 
+from . import _lib
 from .agent import MujocoAgent, SACLearner
 from .env import VecQuadrupedalEnv, apply_dynamic_param
-from .es import PopulationEvaluator, SimpleGA, solutions_to_etg_device
+from .es import PopulationEvaluator, SimpleGA, TrainEpisodeStats, solutions_to_etg_device
 from .etg import ETG_layer, Opt_with_points
 from .replay import ReplayMemory
 from .terrain import make_terrain
@@ -66,7 +72,94 @@ def parser():
                    "param2dynamic_dict -> every env of training, the ES phase and --eval (train.py:302-303); empty = nominal dynamics")
     p.add_argument("--ETG_path", type=str, default="None", help="a pretrained ETG (.npz with `param`, e.g. pretrain's itr_*.npz): its 12 control-point "
                    "offsets seed the ES solver and the first gait (train.py:281-299); a missing file keeps zero offsets.  Not with --load")
+    p.add_argument("--train_eval_envs", type=int, default=0, help="K > 0: every --eval_every_steps, one deterministic episode (at most 601 steps) on each of "
+                   "K envs of a separate handle (run_evaluate_episodes, train.py:370-383) and one JSON record; 0 = no evaluation")
+    p.add_argument("--e_step_growth", type=int, default=0, help="G > 0: every --eval_every_steps, `if e_step < 600: e_step += G` (train.py:384-385; the "
+                   "reference's G is 50); 0 = a fixed --e_step")
+    # ---- the rest of the reference's flags (train.py:452-505), with its defaults
+    p.add_argument("--act_mode", type=str, default="traj", choices=("traj", "pose", "torque"), help="motor mode and act_bound (train.py:279,315-320)")
+    p.add_argument("--normal", type=int, default=1)
+    p.add_argument("--vel_d", type=float, default=0.5)
+    p.add_argument("--reward_p", type=float, default=5)
+    p.add_argument("--ETG", type=int, default=1, help="0: no ETG, the policy's action is the whole residual (needs --ES 0)")
+    p.add_argument("--ETG_T2", type=float, default=0.5)
+    p.add_argument("--ETG_H", type=int, default=20)
+    p.add_argument("--stand", type=float, default=0)
+    p.add_argument("--enable_action_filter", type=int, default=0)
+    for k in ("dis", "motor", "imu", "contact", "ETG"):
+        p.add_argument("--sensor_" + k, type=int, default=1)
+    for k in ("ETG_obs", "footpose", "dynamic", "exforce"):
+        p.add_argument("--sensor_" + k, type=int, default=0)
+    p.add_argument("--sensor_noise", type=int, default=0, help="1: Gaussian sensor noise (SENSOR_NOISE_STDDEV), seeded by --seed")
+    p.add_argument("--RNN_mode", type=str, default="None")
+    p.add_argument("--random_dynamic", type=int, default=0)
+    p.add_argument("--random_force", type=int, default=0)
+    p.add_argument("--x_noise", type=int, default=0)
+    p.add_argument("--render", type=int, default=0)
+    for k, t, d in (("epsilon", float, 0.4), ("gamma", float, 0.95), ("random", int, 0), ("timesteps", int, 5), ("timeinterval", int, 1)):
+        p.add_argument("--" + k, type=t, default=d, help="accepted and ignored, as in the reference")
     return p
+
+
+def check_supported(args):
+    """Options the batched engine does not provide raise before any device work (the make_env rule: honoured or raised, never ignored)."""
+    if args.ETG_H != 20:
+        raise NotImplementedError("--ETG_H %d: the RBF layer width is fixed at 20 in the kernel" % args.ETG_H)
+    if args.ETG_T2 != args.ETG_T:
+        raise NotImplementedError("--ETG_T2 %g != --ETG_T %g: the second ETG period is not provided" % (args.ETG_T2, args.ETG_T))
+    if args.stand != 0:
+        raise NotImplementedError("--stand %g: the stand reward term is not provided" % args.stand)
+    for k in ("ETG_obs", "footpose", "dynamic", "exforce"):
+        if getattr(args, "sensor_" + k):
+            raise NotImplementedError("--sensor_%s 1: this rlschool-only observation block is not provided" % k)
+    if args.RNN_mode not in ("None", "", None):
+        raise NotImplementedError("--RNN_mode %s: recurrent observation modes are not provided" % args.RNN_mode)
+    if args.random_dynamic:
+        raise NotImplementedError("--random_dynamic 1: per-episode dynamics randomisation is not provided")
+    if args.random_force:
+        raise NotImplementedError("--random_force 1: per-episode pushes are not provided in the batched env")
+    if args.x_noise:
+        raise NotImplementedError("--x_noise 1: the device auto-reset starts every episode at x = 0")
+    if args.render:
+        raise NotImplementedError("--render 1: there is no GUI window; --eval 1 --render_dir writes the camera frames")
+
+
+def obs_width(args):
+    """The observation width the --sensor_* flags select (env.observation_dim of the training env)."""
+    from .deploy import obs_dim_of
+    return obs_dim_of(args.sensor_dis, args.sensor_motor, args.sensor_imu, args.sensor_contact, args.sensor_ETG)
+
+
+def check_args(p, args):
+    """The argument errors of main, raised (p.error) before any device work."""
+    if args.ES and not args.ETG:
+        p.error("--ETG 0 with --ES 1: the ES phase searches the ETG, which --ETG 0 turns off")
+    if args.train_eval_envs < 0 or args.e_step_growth < 0:
+        p.error("--train_eval_envs and --e_step_growth must be >= 0")
+    if args.load:
+        import torch
+        have = int(torch.load(args.load, map_location="cpu")["actor_model.l1.weight"].shape[1])
+        if have != obs_width(args):
+            p.error("--load %s: the actor takes %d inputs, but the --sensor_* flags give a %d-wide observation" % (args.load, have, obs_width(args)))
+
+
+def grow_e_step(e_step, growth):
+    """train.py:384-385 with the reference's 50 as `growth`."""
+    if e_step < EVAL_MAX_STEP:
+        e_step += growth
+    return e_step
+
+
+def block_due(total, test_flag, every):
+    """train.py:370-372's test of the evaluation / e_step / checkpoint block after the control step that took the env-step count to `total`:
+    (due, test_flag).  test_flag starts at 1, not at the reference's 0, so the first block (also this loop's first checkpoint) comes at the
+    first multiple of `every`, not after the first iteration.  When `every` is a multiple of the number of envs (the default 1e4 per env),
+    the blocks fall on the iterations where the env-step count reaches each multiple."""
+    if (total + 1) // every >= test_flag:
+        while (total + 1) // every >= test_flag:
+            test_flag += 1
+        return True, test_flag
+    return False, test_flag
 
 
 def etg_prior(ETG_T=0.5, footheight=0.1, steplen=0.05):
@@ -97,41 +190,68 @@ def initial_etg(args):
 
 
 def env_config(args):
-    """The reward weights of the command line (train.py:255-261) go to BOTH the training env and the ES evaluator: ES must optimise the
-    reward SAC is trained on."""
+    """The reward weights of the command line (train.py:255-261) and the ETG period go to BOTH the training env and the ES evaluator: ES
+    must optimise the reward SAC is trained on, with the gait (w, b) is fitted to."""
     return dict(w_torso=args.torso, w_feet=args.feet, w_up=args.up, w_tau=args.tau, w_badfoot=args.badfoot, w_footcontact=args.footcontact,
                 heightfield=make_terrain(args.task_mode, step_y=args.step_y), stuck_termination=1, body_collisions=1,
-                etg_foot_y_inset=args.step_y if args.task_mode == "balancebeam" else 0.0)
+                etg_foot_y_inset=args.step_y if args.task_mode == "balancebeam" else 0.0, etg_T=float(args.ETG_T), etg_T2=float(args.ETG_T))
 
 
-def make_envs(args, env_cfg, policy=None):
+def train_env_config(args):
+    """env_config plus the observation, action and reward flags of this command (the make_env keywords of train.py:305-309).  Joint limits and
+    knee contacts stay off, as in every earlier version of this command (quadrupedal_config turns them on)."""
+    from .env import SENSOR_NOISE_STDDEV, _motor_mode
+    cfg = env_config(args)
+    cfg.update(vel_d=float(args.vel_d), reward_p=float(args.reward_p), obs_normal=int(bool(args.normal)), action_filter=int(bool(args.enable_action_filter)),
+               etg_enabled=int(bool(args.ETG)), motor_mode=_motor_mode(args.act_mode), sensor_dis=int(bool(args.sensor_dis)),
+               sensor_contact=int(bool(args.sensor_contact)), sensor_imu=int(args.sensor_imu), sensor_motor=int(args.sensor_motor), sensor_etg=int(bool(args.sensor_ETG)))
+    if args.sensor_noise:
+        cfg.update(noise_stdev=SENSOR_NOISE_STDDEV, noise_seed=int(args.seed))
+    return cfg
+
+
+def make_envs(args, env_cfg, policy=None, act_bound=None):
     """The training env and the ES phase's PopulationEvaluator (None without --ES), both on the --dynamic_param dynamics."""
     env = apply_dynamic_param(VecQuadrupedalEnv(args.num_envs, auto_reset=True, max_episode_steps=args.e_step, **env_cfg), args.dynamic_param)
     evaluator = None
     if args.ES:
-        evaluator = PopulationEvaluator(args.popsize, args.es_rollouts, max_steps=args.e_step, policy=policy, act_bound=args.act_bound, **env_cfg)
+        evaluator = PopulationEvaluator(args.popsize, args.es_rollouts, max_steps=args.e_step, policy=policy,
+                                        act_bound=args.act_bound if act_bound is None else act_bound, **env_cfg)
         apply_dynamic_param(evaluator.env, args.dynamic_param)
     return env, evaluator
+
+
+def make_eval_env(args, env_cfg, n):
+    """An env of n envs without auto-reset on the training configuration and the --dynamic_param dynamics (--eval, --train_eval_envs)."""
+    return apply_dynamic_param(VecQuadrupedalEnv(n, auto_reset=False, **env_cfg), args.dynamic_param)
 
 
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    check_supported(args)
     torch.manual_seed(args.seed); np.random.seed(args.seed)
     n = args.num_envs
     layer = ETG_layer(args.ETG_T, 0.026, 20, 0.04, np.array([-np.pi / 2, 0]), 0.2, args.ETG_T)
     w0, b0, prior_points = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, Footheight=args.footheight, Steplength=args.steplen)     # train.py:298-299
     w, b = w0, b0
-    env_cfg = env_config(args)
+    env_cfg = train_env_config(args)
     if args.load and args.ETG_path not in ("", "None"):
         p.error("--ETG_path and --load both set the ETG: --load restores (w, b, param) from the .npz next to the checkpoint")
+    if args.eval and not args.load:
+        p.error("--eval 1 evaluates a checkpoint: it needs --load itr_*.pt")
+    check_args(p, args)
+    from .bctrain import act_bound_of
+    bound = act_bound_of(args)                                                                                                    # train.py:315-320
+    # a uniform bound stays a Python scalar: the same float32 products as before the per-motor bounds of --act_mode pose
+    bound = float(bound[0]) if np.all(bound == bound[0]) else torch.as_tensor(bound, dtype=torch.float32, device="cuda")
     if args.eval:
-        if not args.load:
-            p.error("--eval 1 evaluates a checkpoint: it needs --load itr_*.pt")
-        return evaluate(args, env_cfg)
+        return evaluate(args, env_cfg, bound)
     # the evaluator's policy reads `learner` when it runs, so it may be built before the learner
-    env, evaluator = make_envs(args, env_cfg, policy=lambda o: learner.actor.forward(o)[0][0])
-    agent = MujocoAgent(49, 12, seed=args.seed)
+    env, evaluator = make_envs(args, env_cfg, policy=lambda o: learner.actor.forward(o)[0][0], act_bound=bound)
+    eval_env = make_eval_env(args, env_cfg, args.train_eval_envs) if args.train_eval_envs else None
+    od = env.observation_dim
+    agent = MujocoAgent(od, 12, seed=args.seed)
     ETG_best_param, w, b = initial_etg(args)                                                                                      # ES_solver.get_best_param(), train.py:348
     if args.load:
         agent.restore(args.load)
@@ -141,21 +261,26 @@ def main(argv=None):
     if outdir:
         os.makedirs(outdir, exist_ok=True)
     ckpt_every = args.eval_every_steps or int(1e4) * n
-    next_ckpt = ckpt_every
+    test_flag = 1
+    e_step = args.e_step
     learner = SACLearner(agent, args.batch, gamma=GAMMA, tau=TAU, alpha=ALPHA, actor_lr=ACTOR_LR, critic_lr=CRITIC_LR)
-    rpm = ReplayMemory(args.memory, 49, 12, device_cursor=bool(args.graph_iter and args.overlap))
+    rpm = ReplayMemory(args.memory, od, 12, device_cursor=bool(args.graph_iter and args.overlap))
     solver = SimpleGA(12, sigma_init=args.sigma, sigma_decay=args.sigma_decay, sigma_limit=0.005, elite_ratio=0.1, weight_decay=0.005,
                       popsize=args.popsize, param=ETG_best_param.copy())                                                          # train.py:288-295
     obs = env.reset(w, b).clone()
     total, it, last_es, t0 = 0, 0, 0, time.perf_counter()
     s_learn = torch.cuda.Stream(device=env.device)
-    ret_acc = torch.zeros(n, device=env.device); ep_rets = []; last_log = (0, 0.0)
+    # the per-episode statistics of run_train_episode (train.py:150-157,175,359-366): one b2q_train_episode_stats launch per control step in
+    # both loop modes, read and emptied by every log record
+    stats = TrainEpisodeStats(_lib.load(), n, env.device, EVAL_TERMS)
+    last_log = (0, 0.0)
     log = []
     # ---- one whole iteration as ONE CUDA graph (--graph_iter): everything step-dependent lives in device memory — the replay cursor, the learner's
     #      step counter (which also keys the rsample() noise), torch's graph-safe generator for the exploration noise — so the captured launches are
     #      valid for every later step.  The learner runs on its own stream inside the graph, beside the env step, exactly as in the eager loop below.
+    #      The episode step limit is a kernel argument of the captured env step: a new limit (--e_step_growth) drops the graph, and the loop captures
+    #      it again after one eager iteration.
     iter_graph = None
-    ep_sum = torch.zeros((), device=env.device); ep_cnt = torch.zeros((), device=env.device)
     def graph_iteration():
         cur = torch.cuda.current_stream()
         act = learner.actor.forward(obs, mode=1, eps=torch.randn(n, 12, device=env.device))[0][0]     # agent.sample(obs)
@@ -163,13 +288,10 @@ def main(argv=None):
         s_learn.wait_stream(cur)
         with torch.cuda.stream(s_learn):
             learner.learn(*batch_t, graph=False, pull=False)
-        nobs, rew, done, _ = env.step(act * args.act_bound)
+        nobs, rew, done, info = env.step(act * bound)
+        stats.step(rew, done, info, env._stream())
         rpm.append(obs, act, rew, nobs, 1.0 - done.float())
         cur.wait_stream(s_learn)
-        fin = done.float()
-        ret_acc.add_(rew)
-        ep_sum.add_((ret_acc * fin).sum()); ep_cnt.add_(fin.sum())
-        ret_acc.mul_(1.0 - fin)
         obs.copy_(nobs)
     while total < args.max_steps:
         if iter_graph is not None:
@@ -177,8 +299,6 @@ def main(argv=None):
             rpm.advance(n)
             rew, done, losses = env.reward, env.done, learner.losses
             total += n; it += 1
-            if it % args.log_every == 0 and float(ep_cnt) > 0:
-                ep_rets.append(float(ep_sum / ep_cnt)); ep_sum.zero_(); ep_cnt.zero_()
         else:
             if rpm.size() < args.warmup_steps:
                 act = torch.rand(n, 12, device=env.device) * 2 - 1                         # train.py:141-142
@@ -195,15 +315,11 @@ def main(argv=None):
                     for x in batch_t:
                         x.record_stream(s_learn)
                     losses = learner.learn(*batch_t, graph=True, pull=False)
-            nobs, rew, done, info = env.step(act * args.act_bound)
+            nobs, rew, done, info = env.step(act * bound)
+            stats.step(rew, done, info, env._stream())
             rpm.append(obs, act, rew, nobs, 1.0 - done.float())                            # terminal = 1 - done, train.py:148-149,159
             if learning and args.overlap:
                 torch.cuda.current_stream().wait_stream(s_learn)
-            ret_acc += rew
-            fin = done.bool()
-            if it % args.log_every == 0 and bool(fin.any()):
-                ep_rets.append(float(ret_acc[fin].mean()))
-            ret_acc = torch.where(fin, torch.zeros_like(ret_acc), ret_acc)
             obs.copy_(nobs)
             total += n; it += 1
             if rpm.size() >= args.warmup_steps and not (learning and args.overlap):
@@ -223,15 +339,33 @@ def main(argv=None):
             torch.cuda.synchronize()
             el = time.perf_counter() - t0
             rate_int = (total - last_log[0]) / max(el - last_log[1], 1e-9); last_log = (total, el)
+            ep = stats.take()
+            closed = ep["episodes"] + ep["nonfinite_episodes"] > 0
             rec = {"env_steps": total, "iters": it, "env_steps_per_s": total / el, "interval_env_steps_per_s": rate_int, "mean_step_reward": float(rew.mean()), "done_frac": float(done.float().mean()),
-                   "episode_return": ep_rets[-1] if ep_rets else None,
-                   "critic_loss": float(losses[0]) if rpm.size() >= args.warmup_steps else None, "actor_loss": float(losses[1]) if rpm.size() >= args.warmup_steps else None}
+                   "episode_return": ep["return"],
+                   "critic_loss": float(losses[0]) if rpm.size() >= args.warmup_steps else None, "actor_loss": float(losses[1]) if rpm.size() >= args.warmup_steps else None,
+                   "train_episodes": ep["episodes"] if closed else None, "train_nonfinite_episodes": ep["nonfinite_episodes"] if closed else None,
+                   "train_episode_step": ep["length"]}
+            for k in EVAL_TERMS:
+                rec["train_episode_" + k], rec["train_mean_" + k] = ep["terms"][k], ep["mean_terms"][k]
+            rec["train_success_rate"] = ep["success_rate"]
             log.append(rec); print(json.dumps(rec), flush=True)
-        if outdir and total >= next_ckpt:                                               # agent.save + np.savez(w, b, param), train.py:386-390
-            next_ckpt += ckpt_every
-            learner.pull()
-            agent.save(os.path.join(outdir, "itr_%d.pt" % total))
-            np.savez(os.path.join(outdir, "itr_%d.npz" % total), w=w, b=b, param=ETG_best_param)
+        due, test_flag = block_due(total, test_flag, ckpt_every)
+        if due:                                                                         # train.py:370-390, in its order
+            if eval_env is not None:
+                r = run_evaluate_episodes(eval_env, w, b, policy=lambda o: learner.actor.forward(o)[0][0], act_bound=bound, max_step=EVAL_MAX_STEP)
+                rec = eval_record(total, r, e_step)
+                log.append(rec); print(json.dumps(rec), flush=True)
+            if args.e_step_growth:
+                grown = grow_e_step(e_step, args.e_step_growth)
+                if grown != e_step:
+                    e_step = grown
+                    env.set_max_episode_steps(e_step)
+                    iter_graph = None                                                   # the captured env step holds the old limit
+            if outdir:                                                                  # agent.save + np.savez(w, b, param), train.py:386-390
+                learner.pull()
+                agent.save(os.path.join(outdir, "itr_%d.pt" % total))
+                np.savez(os.path.join(outdir, "itr_%d.npz" % total), w=w, b=b, param=ETG_best_param)
         if evaluator is not None and total - last_es >= args.es_every_steps and rpm.size() >= args.warmup_steps:
             last_es = total
             # the incumbent ETG seeds best_reward (train.py:395-396): a sampled individual replaces it only if it is actually better
@@ -265,10 +399,23 @@ def main(argv=None):
             pts = prior_points + ETG_best_param.reshape(-1, 2)                          # train.py:433-437
             w, b, _ = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, w0=w0, b0=b0, points=pts)
             solver.reset(ETG_best_param)
-            obs.copy_(env.reset(w, b)); ret_acc.zero_()      # in place: the captured iteration graph reads and writes these tensors
+            obs.copy_(env.reset(w, b)); stats.restart()     # in place: the captured iteration graph reads and writes these tensors; cut episodes are dropped
     torch.cuda.synchronize()
     learner.pull()
+    if eval_env is not None:
+        eval_env.close()
     return log
+
+
+def eval_record(total, r, e_step):
+    """The eval/* scalars of train.py:376-383 for one run_evaluate_episodes result; e_step is the training episode limit in force."""
+    rec = {"eval_env_steps": total, "eval_episode_reward": r["mean_return"], "eval_episode_step": r["mean_length"]}
+    for k in EVAL_TERMS:
+        rec["eval_episode_" + k] = r["terms"][k]
+        rec["eval_mean_" + k] = r["terms"][k] / r["mean_length"]
+    rec["eval_success_rate"] = r["success_rate"]
+    rec["e_step"] = e_step
+    return rec
 
 
 EVAL_MAX_STEP = 600                                                         # run_evaluate_episodes(agent, env, 600, ...), train.py:445
@@ -312,16 +459,16 @@ def frame_writer(env, args):
     return frame
 
 
-def evaluate(args, env_cfg):
+def evaluate(args, env_cfg, act_bound):
     """--eval 1: one deterministic episode per env of the restored agent and ETG (w, b) on the training env's config, at most
     EVAL_MAX_STEP + 1 control steps (run_evaluate_episodes).  Prints and returns one JSON record."""
-    agent = MujocoAgent(49, 12, seed=args.seed)
+    n = args.eval_envs
+    env = make_eval_env(args, env_cfg, n)
+    agent = MujocoAgent(env.observation_dim, 12, seed=args.seed)
     agent.restore(args.load)
     z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
     w, b = z["w"], z["b"]
-    n = args.eval_envs
-    env = apply_dynamic_param(VecQuadrupedalEnv(n, auto_reset=False, **env_cfg), args.dynamic_param)
-    r = run_evaluate_episodes(env, w, b, policy=agent.predict_batch, act_bound=args.act_bound, max_step=EVAL_MAX_STEP,
+    r = run_evaluate_episodes(env, w, b, policy=agent.predict_batch, act_bound=act_bound, max_step=EVAL_MAX_STEP,
                               render=frame_writer(env, args) if args.render_dir else None)
     rec = {"eval_envs": n, "mean_return": r["mean_return"], "mean_length": r["mean_length"], "terms": r["terms"]}
     print(json.dumps(rec), flush=True)

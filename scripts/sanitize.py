@@ -118,6 +118,15 @@ for dt in (torch.float32, torch.float64):
         st.step(torch.randn(300, device="cuda", dtype=dt), (torch.rand(300, device="cuda") < 0.3).to(torch.uint8), torch.randn(300, 56, device="cuda", dtype=dt),
                 C.c_void_p(torch.cuda.current_stream().cuda_stream))
 ev.evaluate(np.repeat(w[None], 4, 0), np.repeat(b[None], 4, 0), terms=("torso", "up"))
+# training episode statistics: a partial last block (n = 300) in both precisions with the six terms and a count, with 16 terms, and with none
+from paddlerobotics_b200.es import TrainEpisodeStats
+for dt in (torch.float32, torch.float64):
+    for terms, cc in ((("torso", "feet", "up", "tau", "badfoot", "footcontact"), "velx"), (("torso",) * 16, "velx"), ((), None)):
+        ts = TrainEpisodeStats(_lib.load(), 300, torch.device("cuda"), terms, count_col=cc)
+        for _ in range(3):
+            ts.step(torch.randn(300, device="cuda", dtype=dt), (torch.rand(300, device="cuda") < 0.3).to(torch.uint8), torch.randn(300, 56, device="cuda", dtype=dt),
+                    C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        ts.take(); ts.restart()
 # deployment rehearsal: both kernels in both precisions on a partial last block (13 envs x 12 columns), counters past the table (NaN rows),
 # a record shorter than the rollout, and no ETG block
 from paddlerobotics_b200 import deploy
