@@ -150,6 +150,17 @@ int64_t b2q_launch_count(B2QHandle h);
  * value of b2q_create. */
 int b2q_set_max_episode_steps(B2QHandle h, int max_episode_steps);
 
+/* Whole-handle snapshot, for stopping a run and continuing it bit for bit.  The blob holds everything a later b2q_step / b2q_reset
+ * reads: the SoA pool (state, snapshot, snap_obs, param, ETG packs, observation ring, position history, external force, step
+ * counters) and the handle's mutable host fields (max_episode_steps).  It starts with a header: magic, format version, sizes,
+ * precision, N, ring depth, obs_dim, the B2QConfig fields (pointers and device left out) and a hash of the height field.
+ * dst / src are DEVICE pointers of b2q_snapshot_bytes(h) bytes, 16-byte aligned.  Save is stream-ordered with no host sync.  Load
+ * reads the header to the host (one small copy, waited for), returns B2Q_EINVAL for a blob of another configuration, format or size
+ * (b2q_last_error names the first field that differs) and otherwise enqueues the copy of the pool. */
+int64_t b2q_snapshot_bytes(B2QHandle h);
+int b2q_snapshot_save(B2QHandle h, void* dst, void* stream);
+int b2q_snapshot_load(B2QHandle h, const void* src, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -59,6 +59,15 @@ B2QMlpHandle b2q_sac_mlp(B2QSacHandle h, int which);
 float* b2q_sac_grad_ptr(B2QSacHandle h, int which);
 float* b2q_sac_loss_ptr(B2QSacHandle h);
 int64_t b2q_sac_launch_count(B2QSacHandle h);
+/* Learner snapshot: a header (magic, version, sizes, obs_dim, act_dim, batch, gamma, tau, alpha, both learning rates), then the actor,
+ * critic and target parameters, the four Adam moment buffers, the loss buffer and the device step counter with the closing-Adam ticket.
+ * dst / src: DEVICE pointers of b2q_sac_snapshot_bytes(h) bytes, 16-byte aligned.  Save is stream-ordered with no host sync.  Load
+ * reads the header to the host (waited for), returns B2Q_EINVAL for a blob of another shape, hyper-parameter set, format or size
+ * (b2q_sac_last_error names the field), then copies the buffers and rebuilds the bf16 tensor-core operand images with the packer
+ * of b2q_sac_set_params, so the next learn is bit-identical to the saved learner's. */
+int64_t b2q_sac_snapshot_bytes(B2QSacHandle h);
+int b2q_sac_snapshot_save(B2QSacHandle h, void* dst, void* stream);
+int b2q_sac_snapshot_load(B2QSacHandle h, const void* src, void* stream);
 #ifdef __cplusplus
 }
 #endif

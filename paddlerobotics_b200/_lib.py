@@ -33,6 +33,9 @@ SYMBOLS = {
     "b2q_get_step_count": (_i, [_vp, _vp, _vp]),
     "b2q_launch_count": (C.c_int64, [_vp]),
     "b2q_set_max_episode_steps": (_i, [_vp, _i]),
+    "b2q_snapshot_bytes": (C.c_int64, [_vp]),
+    "b2q_snapshot_save": (_i, [_vp, _vp, _vp]),
+    "b2q_snapshot_load": (_i, [_vp, _vp, _vp]),
     # policy / critic MLP forward on wgmma tensor cores — include/b2q_mlp.h
     "b2q_mlp_create": (_i, [_i, _i, _i, _i, C.POINTER(_vp)]),
     "b2q_mlp_destroy": (_i, [_vp]),
@@ -56,6 +59,9 @@ SYMBOLS = {
     "b2q_sac_grad_ptr": (_vp, [_vp, _i]),
     "b2q_sac_loss_ptr": (_vp, [_vp]),
     "b2q_sac_launch_count": (C.c_int64, [_vp]),
+    "b2q_sac_snapshot_bytes": (C.c_int64, [_vp]),
+    "b2q_sac_snapshot_save": (_i, [_vp, _vp, _vp]),
+    "b2q_sac_snapshot_load": (_i, [_vp, _vp, _vp]),
     # ES population fitness — include/b2q_es.h
     "b2q_es_accumulate": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "b2q_es_accumulate_terms": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, C.c_double, _vp, _i, _i, _vp]),

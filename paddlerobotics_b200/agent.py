@@ -263,6 +263,29 @@ class SACLearner:
         # wrap the device bucket without copying (for in-place NCCL all-reduce)
         return torch.as_tensor(_CudaBuf(self.lib.b2q_sac_grad_ptr(self.h, which), n), device=self.agent.device)
 
+    def state_dict(self):
+        """The learner's whole training state as CPU tensors: b2q_sac_snapshot_save (parameters, target, Adam moments, loss buffer, device
+        step counter) and the host step count, which seeds the eager learn() and a captured one."""
+        blob = torch.empty(int(self.lib.b2q_sac_snapshot_bytes(self.h)), dtype=torch.uint8, device=self.agent.device)
+        rc = self.lib.b2q_sac_snapshot_save(self.h, blob.data_ptr(), self._stream())
+        if rc != 0:
+            raise RuntimeError("b2q_sac_snapshot_save: %d %s" % (rc, self.lib.b2q_sac_last_error(self.h).decode()))
+        return {"snapshot": blob.cpu(), "steps": self.steps}
+
+    def load_state_dict(self, sd):
+        """Restores a state_dict() of a learner with the same shapes and hyper-parameters, then pull()s the weights into the agent."""
+        want = int(self.lib.b2q_sac_snapshot_bytes(self.h))
+        blob = sd["snapshot"]
+        if blob.dtype != torch.uint8 or blob.numel() != want:
+            raise ValueError("learner snapshot of %d bytes, this learner's is %d" % (blob.numel() * blob.element_size(), want))
+        blob = blob.to(self.agent.device)
+        rc = self.lib.b2q_sac_snapshot_load(self.h, blob.data_ptr(), self._stream())
+        if rc != 0:
+            raise RuntimeError("b2q_sac_snapshot_load: %d %s" % (rc, self.lib.b2q_sac_last_error(self.h).decode()))
+        self.steps = int(sd["steps"])
+        self.pull()
+        torch.cuda.current_stream(self.agent.device).synchronize()     # `blob` is freed on return
+
     def static_batch(self):
         """The learner's static input tensors (obs, act, rew, next_obs, term) of the CUDA-graph path.  Fill them in place (e.g.
         ReplayMemory.sample_batch(n, out=learner.static_batch())) and pass them to learn(graph=True): no per-step input copies."""

@@ -12,6 +12,7 @@
 #include "b2q_host_common.h"
 #include "b2q_env_view.h"
 #include "b2q_render_internal.h"
+#include "b2q_snapshot.h"
 #include "../../include/b2q_render.h"
 
 using namespace b2q;
@@ -204,6 +205,40 @@ __global__ void b2q_set_state_kernel(P4<T>* st, const T* in, int N) {
 
 thread_local std::string g_create_err;
 
+// ---- env snapshot (b2q_snapshot_*): header + the whole SoA pool
+constexpr uint32_t ENV_SNAP_VERSION = 1;
+struct EnvSnapHeader {
+  char magic[8];
+  uint32_t version, header_bytes;
+  int64_t total_bytes;
+  int32_t precision, num_envs, ring_depth, obs_dim;
+  uint64_t hf_hash;            // FNV-1a of the height field's samples (0 on the plane)
+  int32_t max_episode_steps;   // host field of the handle (b2q_set_max_episode_steps): restored by a load, not compared
+  int32_t pad_;
+  B2QConfig cfg;               // device, hf_host and max_episode_steps zeroed
+};
+#define B2Q_SNAP_FIELD(s, f, name) b2q_snap::Field{name, offsetof(s, f), sizeof(((s*)nullptr)->f)}
+#define B2Q_SNAP_CFG(f) B2Q_SNAP_FIELD(EnvSnapHeader, cfg.f, #f)
+// compared in this order by a load; the first difference is named in the error
+const b2q_snap::Field ENV_SNAP_FIELDS[] = {
+    B2Q_SNAP_FIELD(EnvSnapHeader, magic, "magic"), B2Q_SNAP_FIELD(EnvSnapHeader, version, "version"),
+    B2Q_SNAP_FIELD(EnvSnapHeader, header_bytes, "header size"), B2Q_SNAP_FIELD(EnvSnapHeader, total_bytes, "size"),
+    B2Q_SNAP_FIELD(EnvSnapHeader, precision, "precision"), B2Q_SNAP_FIELD(EnvSnapHeader, num_envs, "num_envs"),
+    B2Q_SNAP_FIELD(EnvSnapHeader, ring_depth, "ring_depth"), B2Q_SNAP_FIELD(EnvSnapHeader, obs_dim, "obs_dim"),
+    B2Q_SNAP_CFG(threads_per_block), B2Q_SNAP_CFG(sim_dt), B2Q_SNAP_CFG(action_repeat), B2Q_SNAP_CFG(solver_iters), B2Q_SNAP_CFG(erp),
+    B2Q_SNAP_CFG(warmstart), B2Q_SNAP_CFG(contact_margin), B2Q_SNAP_CFG(action_interp), B2Q_SNAP_CFG(torque_limit), B2Q_SNAP_CFG(settle_steps),
+    B2Q_SNAP_CFG(etg_enabled), B2Q_SNAP_CFG(action_filter), B2Q_SNAP_CFG(filter_highcut), B2Q_SNAP_CFG(etg_T), B2Q_SNAP_CFG(etg_T2),
+    B2Q_SNAP_CFG(etg_sigma_sq), B2Q_SNAP_CFG(etg_amp), B2Q_SNAP_CFG(etg_phase0), B2Q_SNAP_CFG(etg_phase1), B2Q_SNAP_CFG(w_torso),
+    B2Q_SNAP_CFG(w_feet), B2Q_SNAP_CFG(w_up), B2Q_SNAP_CFG(w_tau), B2Q_SNAP_CFG(w_stand), B2Q_SNAP_CFG(w_badfoot), B2Q_SNAP_CFG(w_footcontact),
+    B2Q_SNAP_CFG(w_done), B2Q_SNAP_CFG(reward_p), B2Q_SNAP_CFG(vel_d), B2Q_SNAP_CFG(foot_radius), B2Q_SNAP_CFG(auto_reset),
+    B2Q_SNAP_CFG(terrain_type), B2Q_SNAP_CFG(hf_nx), B2Q_SNAP_CFG(hf_ny), B2Q_SNAP_CFG(hf_x0), B2Q_SNAP_CFG(hf_y0), B2Q_SNAP_CFG(hf_cell),
+    B2Q_SNAP_CFG(clip_motor_commands), B2Q_SNAP_CFG(max_angle_change), B2Q_SNAP_CFG(sensor_dis), B2Q_SNAP_CFG(sensor_contact),
+    B2Q_SNAP_CFG(sensor_imu), B2Q_SNAP_CFG(sensor_motor), B2Q_SNAP_CFG(sensor_etg), B2Q_SNAP_CFG(obs_normal), B2Q_SNAP_CFG(noise_stdev),
+    B2Q_SNAP_CFG(noise_seed), B2Q_SNAP_CFG(stuck_termination), B2Q_SNAP_CFG(body_collisions), B2Q_SNAP_CFG(motor_mode),
+    B2Q_SNAP_CFG(joint_limits), B2Q_SNAP_CFG(external_force), B2Q_SNAP_CFG(base_damping), B2Q_SNAP_CFG(etg_foot_y_inset),
+    B2Q_SNAP_CFG(knee_contacts), B2Q_SNAP_FIELD(EnvSnapHeader, hf_hash, "height field"),
+};
+
 struct EnvBase {
   B2QConfig cfg;
   int prec;
@@ -224,6 +259,9 @@ struct EnvBase {
   virtual int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
                      int32_t* seg, cudaStream_t s) = 0;
   virtual void view(EnvView* v) const = 0;
+  virtual int64_t snapshot_bytes() const = 0;
+  virtual int snapshot_save(void* dst, cudaStream_t s) = 0;
+  virtual int snapshot_load(const void* src, cudaStream_t s) = 0;
 };
 
 #define CK(call)                                                                      \
@@ -254,6 +292,7 @@ struct EnvT : EnvBase {
     if (d_hf) cudaFree(d_hf);
     if (st_act) cudaFree(st_act);
     if (h_flag) cudaFreeHost(h_flag);
+    if (h_snap) cudaFreeHost(h_snap);
   }
   int grid_lanes() const { return (B.N * 4 + tpb - 1) / tpb; }
 
@@ -268,6 +307,7 @@ struct EnvT : EnvBase {
       T* tmp = (T*)malloc(n * sizeof(T));
       if (!tmp) { err = "host alloc failed"; return B2Q_ENOMEM; }
       for (size_t i = 0; i < n; i++) tmp[i] = (T)c.hf_host[i];
+      hf_hash = b2q_snap::fnv1a(c.hf_host, n * sizeof(double));
       hf_lo = hf_hi = (float)tmp[0];   // height range of the field: the camera rays are clipped to it (b2q_render)
       for (size_t i = 0; i < n; i++) { hf_lo = std::fmin(hf_lo, (float)tmp[i]); hf_hi = std::fmax(hf_hi, (float)tmp[i]); }
       cudaError_t e1 = cudaMalloc(&d_hf, n * sizeof(T));
@@ -290,6 +330,7 @@ struct EnvT : EnvBase {
       }
     }
     CK(cudaHostAlloc((void**)&h_flag, sizeof(int), cudaHostAllocDefault));
+    CK(cudaHostAlloc(&h_snap, b2q_snap::HDR_BYTES, cudaHostAllocDefault));
     CK(cudaMalloc((void**)&d_model, (sizeof(Model<T>) + 15) / 16 * 16));      // padded: the kernels stage it with 16-byte loads
     CK(cudaMemset(d_model, 0, (sizeof(Model<T>) + 15) / 16 * 16));
     CK(cudaMemcpy(d_model, &hm, sizeof(Model<T>), cudaMemcpyHostToDevice));
@@ -299,6 +340,7 @@ struct EnvT : EnvBase {
     // one pool for the SoA env state: [state NS | snap NS | snap_obs 12 | param NP | etg NE | ring Dm*24] packs x N, + step counters
     size_t packs = (size_t)(NS + NS + 12 + NP + NE + Dm * 24 + STUCK_H + 1) * N;
     size_t bytes = packs * sizeof(P4<T>) + (size_t)(N + 1) * sizeof(int);
+    pool_bytes = bytes;
     CK(cudaMalloc(&d_pool, bytes));
     CK(cudaMemset(d_pool, 0, bytes));
     P4<T>* p = (P4<T>*)d_pool;
@@ -440,6 +482,46 @@ struct EnvT : EnvBase {
     return B2Q_OK;
   }
   void set_max_steps(int m) override { cfg.max_episode_steps = m; kc.max_steps = m; }   // kc goes to the step kernel by value
+  // The pool is the whole device state a step or reset reads and writes (the model, default dynamics and height field are fixed at
+  // create); cfg.max_episode_steps (= kc.max_steps) is the one host field that changes after create.  `launches` only counts.
+  size_t pool_bytes = 0;
+  uint64_t hf_hash = 0;
+  void* h_snap = nullptr;   // pinned landing slot of a loaded header
+  int64_t snapshot_bytes() const override { return (int64_t)(b2q_snap::HDR_BYTES + pool_bytes); }
+  EnvSnapHeader snap_header() const {
+    EnvSnapHeader h;
+    std::memset(&h, 0, sizeof h);
+    std::memcpy(h.magic, "B2QENV\0\0", 8);
+    h.version = ENV_SNAP_VERSION; h.header_bytes = (uint32_t)b2q_snap::HDR_BYTES; h.total_bytes = snapshot_bytes();
+    h.precision = prec; h.num_envs = B.N; h.ring_depth = B.Dm; h.obs_dim = obs_dim; h.hf_hash = hf_hash; h.max_episode_steps = cfg.max_episode_steps;
+    h.cfg = cfg; h.cfg.device = 0; h.cfg.hf_host = nullptr; h.cfg.max_episode_steps = 0;
+    return h;
+  }
+  int snapshot_save(void* dst, cudaStream_t s) override {
+    if (!dst || ((size_t)dst & 15)) { err = "b2q_snapshot_save: dst must be a 16-byte aligned device pointer"; return B2Q_EINVAL; }
+    CK(cudaSetDevice(cfg.device));
+    CK(b2q_snap::write_header(snap_header(), dst, s));
+    CK(cudaMemcpyAsync((char*)dst + b2q_snap::HDR_BYTES, d_pool, pool_bytes, cudaMemcpyDeviceToDevice, s));
+    launches++;
+    return B2Q_OK;
+  }
+  int snapshot_load(const void* src, cudaStream_t s) override {
+    if (!src || ((size_t)src & 15)) { err = "b2q_snapshot_load: src must be a 16-byte aligned device pointer"; return B2Q_EINVAL; }
+    CK(cudaSetDevice(cfg.device));
+    // the refusal is a return code, so the header has to reach the host first: one small copy, waited for
+    CK(cudaMemcpyAsync(h_snap, src, sizeof(EnvSnapHeader), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    const EnvSnapHeader mine = snap_header();
+    if (const char* f = b2q_snap::first_difference(h_snap, &mine, ENV_SNAP_FIELDS, (int)(sizeof ENV_SNAP_FIELDS / sizeof ENV_SNAP_FIELDS[0]))) {
+      err = std::string("b2q_snapshot_load: the blob's ") + f + " differs from this handle's";
+      return B2Q_EINVAL;
+    }
+    const int m = static_cast<const EnvSnapHeader*>(h_snap)->max_episode_steps;
+    if (m < 0) { err = "b2q_snapshot_load: the blob's max_episode_steps is negative"; return B2Q_EINVAL; }
+    CK(cudaMemcpyAsync(d_pool, (const char*)src + b2q_snap::HDR_BYTES, pool_bytes, cudaMemcpyDeviceToDevice, s));
+    set_max_steps(m);
+    return B2Q_OK;
+  }
   void view(EnvView* v) const override {
     v->N = B.N; v->obs_dim = obs_dim; v->elem_size = (int)sizeof(T); v->device = cfg.device; v->step_count = B.step_count; v->model = d_model;
   }
@@ -528,6 +610,9 @@ int b2q_set_max_episode_steps(B2QHandle h, int m) {
   h->impl->set_max_steps(m);
   return B2Q_OK;
 }
+int64_t b2q_snapshot_bytes(B2QHandle h) { return h ? h->impl->snapshot_bytes() : B2Q_EINVAL; }
+int b2q_snapshot_save(B2QHandle h, void* dst, void* s) { return h ? h->impl->snapshot_save(dst, (cudaStream_t)s) : B2Q_EINVAL; }
+int b2q_snapshot_load(B2QHandle h, const void* src, void* s) { return h ? h->impl->snapshot_load(src, (cudaStream_t)s) : B2Q_EINVAL; }
 int b2q_render(B2QHandle h, const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int width, int height, uint8_t* rgba,
                float* depth, int32_t* seg, void* stream) {
   return h ? h->impl->render(state, env_ids, V, view, proj, width, height, rgba, depth, seg, (cudaStream_t)stream) : B2Q_EINVAL;

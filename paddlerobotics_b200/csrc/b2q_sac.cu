@@ -21,6 +21,7 @@
 #include "b2q_mlp_internal.h"
 #include "b2q_philox.cuh"
 #include "b2q_tc.cuh"
+#include "b2q_snapshot.h"
 
 using namespace b2q_tc;
 typedef __nv_bfloat16 bf16;
@@ -529,6 +530,54 @@ int actor_backward(B2QSac* s, cudaStream_t st) {
   cudaStreamWaitEvent(st, s->ev_aux[3], 0);
   return rc;
 }
+// the bf16 tensor-core operand images of all three parameter groups from the f32 parameters (b2q_sac_set_params, b2q_sac_snapshot_load)
+int repack_all(B2QSac* s, cudaStream_t st) {
+  const int na = (int)s->an.n, nc = (int)(2 * s->cn.n);
+  pdl_launch(k_pack, dim3((na + 255) / 256), dim3(256), 0, st, s->p_actor, na, dst_of(s, NETS_ACTOR));
+  pdl_launch(k_pack, dim3((nc + 255) / 256), dim3(256), 0, st, s->p_critic, nc, dst_of(s, NETS_CRITIC));
+  pdl_launch(k_pack, dim3((nc + 255) / 256), dim3(256), 0, st, s->p_target, nc, dst_of(s, NETS_TARGET));
+  s->launches += 3;
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
+// ---- learner snapshot (b2q_sac_snapshot_*): header, then the float buffers of sac_parts() in order, then d_step [2] (padded to 16 bytes)
+constexpr uint32_t SAC_SNAP_VERSION = 1;
+struct SacSnapHeader {
+  char magic[8];
+  uint32_t version, header_bytes;
+  int64_t total_bytes;
+  int32_t obs_dim, act_dim, batch, pad_;
+  float gamma, tau, alpha, actor_lr, critic_lr;
+};
+#define B2Q_SAC_FIELD(f, name) b2q_snap::Field{name, offsetof(SacSnapHeader, f), sizeof(((SacSnapHeader*)nullptr)->f)}
+const b2q_snap::Field SAC_SNAP_FIELDS[] = {
+    B2Q_SAC_FIELD(magic, "magic"), B2Q_SAC_FIELD(version, "version"), B2Q_SAC_FIELD(header_bytes, "header size"), B2Q_SAC_FIELD(total_bytes, "size"),
+    B2Q_SAC_FIELD(obs_dim, "obs_dim"), B2Q_SAC_FIELD(act_dim, "act_dim"), B2Q_SAC_FIELD(batch, "batch"), B2Q_SAC_FIELD(gamma, "gamma"),
+    B2Q_SAC_FIELD(tau, "tau"), B2Q_SAC_FIELD(alpha, "alpha"), B2Q_SAC_FIELD(actor_lr, "actor_lr"), B2Q_SAC_FIELD(critic_lr, "critic_lr"),
+};
+struct SacPart { float* p; size_t n; };
+// actor, critic, target, Adam m/v of the actor and of the critic, the loss buffer
+void sac_parts(const B2QSac* s, SacPart out[8]) {
+  const size_t na = s->an.n, nc = 2 * s->cn.n;
+  out[0] = {s->p_actor, na}; out[1] = {s->p_critic, nc}; out[2] = {s->p_target, nc}; out[3] = {s->m_a, na};
+  out[4] = {s->v_a, na}; out[5] = {s->m_c, nc}; out[6] = {s->v_c, nc}; out[7] = {s->losses, 4};
+}
+size_t sac_payload_floats(const B2QSac* s) {   // the blob's size follows the part list that save and load walk
+  SacPart parts[8]; sac_parts(s, parts);
+  size_t n = 0;
+  for (const SacPart& q : parts) n += q.n;
+  return n;
+}
+int64_t sac_snapshot_bytes(const B2QSac* s) { return (int64_t)(b2q_snap::HDR_BYTES + sac_payload_floats(s) * sizeof(float) + 16); }
+SacSnapHeader sac_header(const B2QSac* s) {
+  SacSnapHeader h;
+  std::memset(&h, 0, sizeof h);
+  std::memcpy(h.magic, "B2QSAC\0\0", 8);
+  h.version = SAC_SNAP_VERSION; h.header_bytes = (uint32_t)b2q_snap::HDR_BYTES; h.total_bytes = sac_snapshot_bytes(s);
+  h.obs_dim = s->D; h.act_dim = s->A; h.batch = s->B; h.gamma = s->gamma; h.tau = s->tau; h.alpha = s->alpha; h.actor_lr = s->lr_a; h.critic_lr = s->lr_c;
+  return h;
+}
+
 }  // namespace
 
 extern "C" {
@@ -598,12 +647,7 @@ int b2q_sac_set_params(B2QSacHandle s, const float* actor, const float* critic, 
   if (critic) cudaMemcpyAsync(s->p_critic, critic, 2 * s->cn.n * sizeof(float), cudaMemcpyDeviceToDevice, st);
   if (target) cudaMemcpyAsync(s->p_target, target, 2 * s->cn.n * sizeof(float), cudaMemcpyDeviceToDevice, st);
   else if (critic) cudaMemcpyAsync(s->p_target, critic, 2 * s->cn.n * sizeof(float), cudaMemcpyDeviceToDevice, st);   // MujocoAgent: sync_target(decay=0)
-  const int na = (int)s->an.n, nc = (int)(2 * s->cn.n);
-  pdl_launch(k_pack, dim3((na + 255) / 256), dim3(256), 0, st, s->p_actor, na, dst_of(s, NETS_ACTOR));
-  pdl_launch(k_pack, dim3((nc + 255) / 256), dim3(256), 0, st, s->p_critic, nc, dst_of(s, NETS_CRITIC));
-  pdl_launch(k_pack, dim3((nc + 255) / 256), dim3(256), 0, st, s->p_target, nc, dst_of(s, NETS_TARGET));
-  s->launches += 3;
-  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+  return repack_all(s, st);
 }
 int b2q_sac_get_params(B2QSacHandle s, float* actor, float* critic, float* target, void* stream) {
   if (!s) return -1;
@@ -741,6 +785,48 @@ int b2q_sac_bc_learn(B2QSacHandle s, const float* obs, const float* ref_obs, int
 B2QMlpHandle b2q_sac_mlp(B2QSacHandle s, int which) { return !s ? nullptr : (which == 0 ? s->mlp_actor : (which == 1 ? s->mlp_critic : s->mlp_target)); }
 float* b2q_sac_grad_ptr(B2QSacHandle s, int which) { return !s ? nullptr : (which == 1 ? s->g_critic : s->g_actor); }   // which == 2: the flat bucket (starts at the actor part)
 float* b2q_sac_loss_ptr(B2QSacHandle s) { return s ? s->losses : nullptr; }
+
+int64_t b2q_sac_snapshot_bytes(B2QSacHandle s) { return s ? sac_snapshot_bytes(s) : -1; }
+int b2q_sac_snapshot_save(B2QSacHandle s, void* dst, void* stream) {
+  if (!s) return -1;
+  if (!dst || ((size_t)dst & 15)) { s->err = "b2q_sac_snapshot_save: dst must be a 16-byte aligned device pointer"; return -1; }
+  cudaSetDevice(s->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (b2q_snap::write_header(sac_header(s), dst, st) != cudaSuccess) { s->err = "b2q_sac_snapshot_save: header store failed"; return -2; }
+  char* o = (char*)dst + b2q_snap::HDR_BYTES;
+  SacPart parts[8]; sac_parts(s, parts);
+  for (const SacPart& q : parts) { cudaMemcpyAsync(o, q.p, q.n * sizeof(float), cudaMemcpyDeviceToDevice, st); o += q.n * sizeof(float); }
+  cudaMemsetAsync(o, 0, 16, st);                     // the tail's padding too: equal learners give equal blobs
+  cudaMemcpyAsync(o, s->d_step, 2 * sizeof(int), cudaMemcpyDeviceToDevice, st);
+  s->launches++;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { s->err = cudaGetErrorString(e); return -2; }
+  return 0;
+}
+int b2q_sac_snapshot_load(B2QSacHandle s, const void* src, void* stream) {
+  if (!s) return -1;
+  if (!src || ((size_t)src & 15)) { s->err = "b2q_sac_snapshot_load: src must be a 16-byte aligned device pointer"; return -1; }
+  cudaSetDevice(s->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  // the refusal is a return code, so the header has to reach the host first: one small copy, waited for
+  SacSnapHeader got;
+  if (cudaMemcpyAsync(&got, src, sizeof got, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
+    s->err = "b2q_sac_snapshot_load: header read failed"; return -2;
+  }
+  const SacSnapHeader mine = sac_header(s);
+  if (const char* f = b2q_snap::first_difference(&got, &mine, SAC_SNAP_FIELDS, (int)(sizeof SAC_SNAP_FIELDS / sizeof SAC_SNAP_FIELDS[0]))) {
+    s->err = std::string("b2q_sac_snapshot_load: the blob's ") + f + " differs from this learner's";
+    return -1;
+  }
+  const char* o = (const char*)src + b2q_snap::HDR_BYTES;
+  SacPart parts[8]; sac_parts(s, parts);
+  for (const SacPart& q : parts) { cudaMemcpyAsync(q.p, o, q.n * sizeof(float), cudaMemcpyDeviceToDevice, st); o += q.n * sizeof(float); }
+  cudaMemcpyAsync(s->d_step, o, 2 * sizeof(int), cudaMemcpyDeviceToDevice, st);
+  // the gradient bucket is not in the blob: every learn clears it before use, and a phase 2 without a phase 0 clears the actor part when
+  // this flag is set, so the next step reads the same zeros the saved learner would have
+  s->actor_grad_dirty = true;
+  return repack_all(s, st);
+}
 
 
 }  // extern "C"

@@ -130,6 +130,28 @@ class VecQuadrupedalEnv:
         _check(self.lib, self.h, self.lib.b2q_set_max_episode_steps(self.h, int(m)), "b2q_set_max_episode_steps")
         self.cfg.max_episode_steps = int(m)
 
+    def state_dict(self):
+        """Everything a later step or reset reads (b2q_snapshot_save: the device pool and the episode step limit), plus the last step's
+        outputs, as CPU tensors."""
+        blob = torch.empty(int(self.lib.b2q_snapshot_bytes(self.h)), dtype=torch.uint8, device=self.device)
+        _check(self.lib, self.h, self.lib.b2q_snapshot_save(self.h, blob.data_ptr(), self._stream()), "b2q_snapshot_save")
+        return {"snapshot": blob.cpu(), "max_episode_steps": int(self.cfg.max_episode_steps), "obs": self.obs.cpu(), "reward": self.reward.cpu(),
+                "done": self.done.cpu(), "info": self.info.cpu()}
+
+    def load_state_dict(self, sd):
+        """Restores a state_dict() of an env built with the same configuration; raises ValueError for a blob of another size and
+        RuntimeError (naming the first differing field) for one of another configuration."""
+        want = int(self.lib.b2q_snapshot_bytes(self.h))
+        blob = sd["snapshot"]
+        if blob.dtype != torch.uint8 or blob.numel() != want:
+            raise ValueError("env snapshot of %d bytes, this env's is %d" % (blob.numel() * blob.element_size(), want))
+        blob = blob.to(self.device)
+        _check(self.lib, self.h, self.lib.b2q_snapshot_load(self.h, blob.data_ptr(), self._stream()), "b2q_snapshot_load")
+        self.cfg.max_episode_steps = int(sd["max_episode_steps"])
+        for k in ("obs", "reward", "done", "info"):
+            getattr(self, k).copy_(sd[k])
+        torch.cuda.current_stream(self.device).synchronize()     # `blob` is freed on return
+
     def get_camera_image(self, width=640, height=480, env_ids=None, view=None, proj=None):
         """Ray-cast camera images of the current state (b2q_render, include/b2q_render.h): view v shows env env_ids[v] (default
         every env).  view / proj: [16] (one matrix for every view) or [V,16] column-major pybullet matrices; None = the follow

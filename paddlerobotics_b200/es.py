@@ -9,6 +9,7 @@
   inside the CUDA step kernel; per-env returns are frozen at the first `done`; fitness = mean over rollouts
   (`b2q_es_fitness`); shards are concatenated with ONE all-gather (NCCL on GPUs, gloo in the CPU tests).
 """
+import copy
 import ctypes as C
 
 import numpy as np
@@ -38,6 +39,15 @@ class SimpleGA:
         self.best_reward = 0
         self.first_iteration = True
         self.forget_best, self.weight_decay = forget_best, weight_decay
+
+    def state_dict(self):
+        """The solver's attributes (sigma, elite set, best parameters, ...) and NumPy's global RNG state, which ask() draws from."""
+        return {"attrs": copy.deepcopy(vars(self)), "np_random": np.random.get_state()}
+
+    def load_state_dict(self, sd):
+        """Restores a state_dict(), NumPy's global RNG state included: the next ask() equals the saved solver's."""
+        self.__dict__.update(copy.deepcopy(sd["attrs"]))
+        np.random.set_state(sd["np_random"])
 
     def reset(self, param):
         self.best_param = np.copy(param)
@@ -432,6 +442,12 @@ class TrainEpisodeStats:
     def restart(self):
         """Drops the running episodes (after a hard env.reset): the next step starts a new episode in every env."""
         self.run.zero_()
+
+    def state_dict(self):
+        return {"run": self.run.cpu(), "win": self.win.cpu()}
+
+    def load_state_dict(self, sd):
+        self.run.copy_(sd["run"]); self.win.copy_(sd["win"])
 
     def take(self):
         """The window's means over its finite episodes, then an empty window.  {episodes, nonfinite_episodes, return, length, terms: {term:

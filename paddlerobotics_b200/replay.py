@@ -50,6 +50,32 @@ class ReplayMemory:
     def __len__(self):
         return self.size()
 
+    def state_dict(self):
+        """The ring's rows up to the fill level, the device cursor [position, fill level, samples] (None in host-cursor mode) and the host
+        mirrors, as CPU tensors."""
+        self._refresh()
+        n = self._curr_size
+        return {"max_size": self.max_size, "obs_dim": self.obs_dim, "act_dim": self.act_dim, "obs": self.obs[:n].cpu(), "action": self.action[:n].cpu(),
+                "reward": self.reward[:n].cpu(), "next_obs": self.next_obs[:n].cpu(), "terminal": self.terminal[:n].cpu(),
+                "cursor": None if self.cursor is None else self.cursor.cpu(), "pos": self._curr_pos, "size": n, "samples": self._samples}
+
+    def load_state_dict(self, sd):
+        """Restores a state_dict() into this memory's buffers (same capacity, widths and cursor mode); rows past the fill level are zeroed."""
+        if (sd["max_size"], sd["obs_dim"], sd["act_dim"]) != (self.max_size, self.obs_dim, self.act_dim):
+            raise ValueError("replay memory state of shape %s, this memory is %s" % ((sd["max_size"], sd["obs_dim"], sd["act_dim"]), (self.max_size, self.obs_dim, self.act_dim)))
+        if (sd["cursor"] is None) != (self.cursor is None):
+            raise ValueError("replay memory state and this memory differ in cursor mode (device cursor: %s here)" % (self.cursor is not None))
+        n = int(sd["size"])
+        for k in ("obs", "action", "reward", "next_obs", "terminal"):
+            buf = getattr(self, k)
+            buf[:n].copy_(sd[k])
+            buf[n:].zero_()
+        if self.cursor is not None:
+            self.cursor.copy_(sd["cursor"])
+        self._curr_pos, self._curr_size, self._samples = int(sd["pos"]), n, int(sd["samples"])
+        self._stale = False
+        torch.cuda.current_stream(self.device).synchronize()     # the CPU sources must not be freed before the copies ran
+
     def append_masked(self, obs, act, reward, next_obs, terminal, mask):
         """Appends the rows i with mask[i] != 0, in row order (one row per env whose transition is kept, e.g. the envs still in their
         first episode).  The number of rows written never reaches the host (b2q_rpm_append_masked_cursor): no sync, and in device-cursor

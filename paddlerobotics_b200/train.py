@@ -9,6 +9,7 @@ The reference's flags are honoured or refused before any device work (check_supp
 
     python -m paddlerobotics_b200.train --num_envs 4096 --max_steps 2000000 --ES 1
     python -m paddlerobotics_b200.train --train_eval_envs 16 --e_step_growth 50 --outdir train_log
+    python -m paddlerobotics_b200.train --outdir ckpt --save_state 1; python -m paddlerobotics_b200.train --outdir ckpt --resume ckpt/exp0/state.pt --max_steps N
 """
 import argparse
 import json
@@ -74,6 +75,11 @@ def parser():
                    "offsets seed the ES solver and the first gait (train.py:281-299); a missing file keeps zero offsets.  Not with --load")
     p.add_argument("--train_eval_envs", type=int, default=0, help="K > 0: every --eval_every_steps, one deterministic episode (at most 601 steps) on each of "
                    "K envs of a separate handle (run_evaluate_episodes, train.py:370-383) and one JSON record; 0 = no evaluation")
+    p.add_argument("--save_state", type=int, default=0, help="1: write the whole training state to <outdir>/<suffix>/state.pt after every evaluation block "
+                   "(after its iteration's ES phase) and when --max_steps is reached, replacing the previous file atomically (needs --outdir)")
+    p.add_argument("--resume", type=str, default="", help="a state.pt of --save_state: continue that run with its arguments (bit for bit until the first learn, then as close as two "
+                   "uninterrupted runs: the learner sums with f32 atomics); only --max_steps, "
+                   "--log_every, --outdir, --suffix and --save_state may be given with other values")
     p.add_argument("--e_step_growth", type=int, default=0, help="G > 0: every --eval_every_steps, `if e_step < 600: e_step += G` (train.py:384-385; the "
                    "reference's G is 50); 0 = a fixed --e_step")
     # ---- the rest of the reference's flags (train.py:452-505), with its defaults
@@ -141,6 +147,47 @@ def check_args(p, args):
         have = int(torch.load(args.load, map_location="cpu")["actor_model.l1.weight"].shape[1])
         if have != obs_width(args):
             p.error("--load %s: the actor takes %d inputs, but the --sensor_* flags give a %d-wide observation" % (args.load, have, obs_width(args)))
+
+
+RESUME_FREE = ("max_steps", "log_every", "outdir", "suffix", "save_state", "resume")     # the flags a --resume may change
+
+
+def resume_args(p, argv, saved):
+    """The arguments of a --resume run: the saved run's, with the RESUME_FREE flags of this command line.  Any other flag given on the
+    command line with a value other than the saved one is an argument error (p.error) naming the flags, as are --load, --ETG_path and
+    --eval 1, which set what the state restores."""
+    q = parser()
+    for a in q._actions:
+        a.default = argparse.SUPPRESS
+    given = vars(q.parse_args(argv))
+    conflicts = [f for f, bad in (("--load", given.get("load", "")), ("--ETG_path", given.get("ETG_path", "None") not in ("", "None")),
+                                  ("--eval 1", given.get("eval", 0))) if bad]
+    if conflicts:
+        p.error("--resume restores the agent, the ETG and the training loop: it cannot be combined with %s" % ", ".join(conflicts))
+    differ = sorted(k for k, v in given.items() if k not in RESUME_FREE and v != saved.get(k))
+    if differ:
+        p.error("--resume %s: these arguments differ from the saved run's: %s" % (given["resume"], ", ".join("--" + k for k in differ)))
+    args = argparse.Namespace(**saved)
+    for k in RESUME_FREE:
+        if k in given:
+            setattr(args, k, given[k])
+    return args
+
+
+def write_atomic(path, obj):
+    """torch.save(obj) to path through a temporary file that is flushed, fsynced and renamed over it: a crash mid-write leaves the
+    previous file intact."""
+    tmp = path + ".tmp"
+    with open(tmp, "wb") as f:
+        torch.save(obj, f)
+        f.flush()
+        os.fsync(f.fileno())
+    os.replace(tmp, path)
+    fd = os.open(os.path.dirname(os.path.abspath(path)), os.O_RDONLY)
+    try:
+        os.fsync(fd)                                                        # the rename itself
+    finally:
+        os.close(fd)
 
 
 def grow_e_step(e_step, growth):
@@ -229,6 +276,12 @@ def make_eval_env(args, env_cfg, n):
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    state = None
+    if args.resume:
+        state = torch.load(args.resume, map_location="cpu", weights_only=False)
+        args = resume_args(p, argv, state["args"])
+    if args.save_state and not args.outdir:
+        p.error("--save_state 1 writes <outdir>/<suffix>/state.pt: it needs --outdir")
     check_supported(args)
     torch.manual_seed(args.seed); np.random.seed(args.seed)
     n = args.num_envs
@@ -236,6 +289,10 @@ def main(argv=None):
     w0, b0, prior_points = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, Footheight=args.footheight, Steplength=args.steplen)     # train.py:298-299
     w, b = w0, b0
     env_cfg = train_env_config(args)
+    run_args = dict(vars(args))                      # what a --save_state file records
+    if state is not None:
+        args = argparse.Namespace(**run_args)
+        args.load, args.ETG_path = "", "None"        # the state supersedes the saved run's starting agent and ETG
     if args.load and args.ETG_path not in ("", "None"):
         p.error("--ETG_path and --load both set the ETG: --load restores (w, b, param) from the .npz next to the checkpoint")
     if args.eval and not args.load:
@@ -281,6 +338,24 @@ def main(argv=None):
     #      The episode step limit is a kernel argument of the captured env step: a new limit (--e_step_growth) drops the graph, and the loop captures
     #      it again after one eager iteration.
     iter_graph = None
+    if state is not None:
+        env.load_state_dict(state["env"]); learner.load_state_dict(state["learner"]); rpm.load_state_dict(state["rpm"])
+        stats.load_state_dict(state["stats"]); solver.load_state_dict(state["solver"])
+        obs.copy_(state["obs"])
+        L = state["loop"]
+        total, it, last_es, test_flag, e_step, last_log = L["total"], L["it"], L["last_es"], L["test_flag"], L["e_step"], (L["last_log_total"], 0.0)
+        ETG_best_param, w, b = state["ETG_best_param"], state["w"], state["b"]
+        losses = learner.losses
+        torch.set_rng_state(state["torch_rng"]); torch.cuda.set_rng_state(state["cuda_rng"], env.device)
+
+    def save_state():
+        torch.cuda.synchronize()
+        write_atomic(os.path.join(outdir, "state.pt"), {
+            "args": run_args, "env": env.state_dict(), "learner": learner.state_dict(), "rpm": rpm.state_dict(), "stats": stats.state_dict(),
+            "solver": solver.state_dict(), "obs": obs.cpu(), "ETG_best_param": np.array(ETG_best_param), "w": np.array(w), "b": np.array(b),
+            "loop": {"total": total, "it": it, "last_es": last_es, "test_flag": test_flag, "e_step": e_step, "last_log_total": last_log[0]},
+            "graph": iter_graph is not None, "torch_rng": torch.get_rng_state(), "cuda_rng": torch.cuda.get_rng_state(env.device)})
+
     def graph_iteration():
         cur = torch.cuda.current_stream()
         act = learner.actor.forward(obs, mode=1, eps=torch.randn(n, 12, device=env.device))[0][0]     # agent.sample(obs)
@@ -293,6 +368,24 @@ def main(argv=None):
         rpm.append(obs, act, rew, nobs, 1.0 - done.float())
         cur.wait_stream(s_learn)
         obs.copy_(nobs)
+    def capture_iteration():
+        torch.cuda.synchronize()
+        cap = torch.cuda.Stream(device=env.device)
+        cap.wait_stream(torch.cuda.current_stream())
+        g = torch.cuda.CUDAGraph()
+        mirrors = (rpm._curr_pos, rpm._curr_size, rpm._samples)
+        with torch.cuda.graph(g, stream=cap):
+            graph_iteration()
+        rpm._curr_pos, rpm._curr_size, rpm._samples = mirrors     # capture records launches, it does not run them: the ring has not moved
+        torch.cuda.current_stream().wait_stream(cap)
+        return g
+    if state is not None and state["graph"]:
+        # the saved run was replaying its captured iteration: capture it again, without the eager iteration that precedes a first capture
+        # (its exploration noise would come from seed=it+1, not from torch's generator).  The captured learn() takes learner.steps + 1 as its
+        # seed, and the saved run's graph holds the value learner.steps had after its capture, which replays leave unchanged.
+        learner.steps -= 1
+        learner.static_batch()     # allocated eagerly, as the uninterrupted run's eager iterations did: not from the graph's pool
+        iter_graph = capture_iteration()
     while total < args.max_steps:
         if iter_graph is not None:
             iter_graph.replay()
@@ -326,15 +419,7 @@ def main(argv=None):
                 losses = learner.learn(*rpm.sample_batch(args.batch, out=learner.static_batch()), graph=True, pull=False)   # one update per control step, train.py:163-169
             if args.graph_iter and args.overlap and learning and it % args.log_every != 0:
                 # warm-up is over and one eager learning iteration has run: capture the iteration once
-                torch.cuda.synchronize()
-                cap = torch.cuda.Stream(device=env.device)
-                cap.wait_stream(torch.cuda.current_stream())
-                iter_graph = torch.cuda.CUDAGraph()
-                mirrors = (rpm._curr_pos, rpm._curr_size, rpm._samples)
-                with torch.cuda.graph(iter_graph, stream=cap):
-                    graph_iteration()
-                rpm._curr_pos, rpm._curr_size, rpm._samples = mirrors     # capture records launches, it does not run them: the ring has not moved
-                torch.cuda.current_stream().wait_stream(cap)
+                iter_graph = capture_iteration()
         if it % args.log_every == 0:
             torch.cuda.synchronize()
             el = time.perf_counter() - t0
@@ -400,6 +485,10 @@ def main(argv=None):
             w, b, _ = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, w0=w0, b0=b0, points=pts)
             solver.reset(ETG_best_param)
             obs.copy_(env.reset(w, b)); stats.restart()     # in place: the captured iteration graph reads and writes these tensors; cut episodes are dropped
+        if due and args.save_state:
+            save_state()
+    if args.save_state:
+        save_state()
     torch.cuda.synchronize()
     learner.pull()
     if eval_env is not None:
