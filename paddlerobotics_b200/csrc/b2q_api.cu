@@ -620,10 +620,10 @@ int b2q_render(B2QHandle h, const void* state, const int32_t* env_ids, int V, co
 
 #ifdef B2Q_REGION_CLOCKS
 // Debug ABI of the region-clock build only (not in include/b2q.h, absent from the product library): waits for the device, copies the
-// first n_warps rows of the step kernel's region clocks to `out` ([n_warps][8] u64: the RC_* regions of b2q_sim.cuh, entry-to-exit
+// first n_warps rows of the step kernel's region clocks to `out` ([n_warps][12] u64: the RC_* regions of b2q_sim.cuh, entry-to-exit
 // cycles, launches; may be NULL) and zeroes every row when `clear` is set.
 int b2q_region_clocks(int device, uint64_t* out, int n_warps, int clear) {
-  static_assert(RC_COLS == 8, "the row layout documented above");
+  static_assert(RC_COLS == 12, "the row layout documented above");
   if (n_warps < 0 || n_warps > RC_MAX_WARPS) return B2Q_EINVAL;
   if (cudaSetDevice(device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) return B2Q_ECUDA;
   const size_t bytes = (size_t)n_warps * RC_COLS * sizeof(unsigned long long);

@@ -82,8 +82,9 @@ template <typename T> B2Q_HD void philox_normal4(uint64_t seed, uint32_t c0, uin
 // reciprocal: one MUFU.RCP + one Newton step on the GPU (no slow path / branch); exact division elsewhere.  Measured exhaustively on H100
 // (tests/gpu_probe): for every normal x with |x| <= 2^126 the device result is the correctly rounded 1/x, the host's.  The edges follow
 // from rcp.approx.ftz: x = +-0, +-inf and subnormal x give NaN (the Newton step computes 0 * inf or inf - inf), |x| > 2^126 gives a
-// signed zero instead of the subnormal 1/x.  No caller reaches them: det of the 3x3 joint-space block and W_ii of an active contact
-// row are positive and far inside the normal range, and sh / th runs only for th >= 1e-4.
+// signed zero instead of the subnormal 1/x.  No caller uses them: det of the 3x3 joint-space block and W_ii of an active contact
+// row are positive and far inside the normal range, and 1/th is used only for th >= 1e-4 (the substep computes 1/W_ii of inactive rows and
+// 1/th for every th, and selects them away).
 #if defined(__CUDA_ARCH__)
 B2Q_HD float m_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return fmaf(r, fmaf(-x, r, 1.0f), r); }
 #else

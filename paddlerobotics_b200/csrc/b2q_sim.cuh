@@ -102,7 +102,9 @@ template <typename T> B2Q_HD void sincos_t(T a, T& s, T& c) { m_sincos(a, s, c);
 // Region clocks of the step kernel, compiled in only with -DB2Q_REGION_CLOCKS (scripts/step_regions.py builds that library apart from
 // the product one).  A mark reads clock64(), charges the cycles since the previous mark to the region that ends there and opens the next.
 // The product build expands every mark to nothing.
-enum { RC_PROLOGUE, RC_PRE_SWEEP, RC_SWEEP, RC_POST_SWEEP, RC_BETWEEN, RC_EPILOGUE, RC_N };
+// The part of a substep before the sweep is split in five: PD and kinematics, bias forces and composite inertias, Schur reduction and
+// Cholesky (with the unconstrained velocities), contact rows, and the Delassus exchange.
+enum { RC_PROLOGUE, RC_PD_KIN, RC_BIAS_INERTIA, RC_SCHUR_CHOL, RC_CONTACT_ROWS, RC_DELASSUS, RC_SWEEP, RC_POST_SWEEP, RC_BETWEEN, RC_EPILOGUE, RC_N };
 #if defined(B2Q_REGION_CLOCKS) && defined(__CUDA_ARCH__)
 #define B2Q_MARK(cm, region) (cm).mark(region)
 #else
@@ -213,7 +215,16 @@ B2Q_HD void etg_act_leg(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, co
 // Scratch layout: Ya[36][6] | blk[4][45] | vec[36][4] | W[36][36].
 constexpr int RPL = 9, NRW = 4 * RPL;
 constexpr int SCRATCH_FLOATS = NRW * 6 + 4 * 45 + NRW * 4 + NRW * NRW;
-constexpr int SCRATCH_FAST = 272;   // the default body's exchange area: Y^T [6][12] | vectors [4][12] | active [4] (+pad) | W' [12][12]
+// Parking area of the default body, after its exchange area: per lane the Cholesky factor (21) and reciprocal diagonal (6), the base
+// rotation (9), the joint-space contact Jacobian (9) and M_k^-1 (6, symmetric) of the substep, which only the impulse application after
+// the sweep reads again.  Stored before the sweep and loaded after it (as are the lane's own Y rows, from the exchange area), they stay
+// out of the registers that the sweep's Delassus matrix fills.  Value i of lane k is at SCRATCH_EXCHANGE + 4 i + k: the four lanes of a
+// robot use four adjacent banks, and a robot's scratch size is 4 times an odd number (mod 32 banks), so a warp's 32 float accesses hit 32
+// different banks.
+constexpr int PARK = 51, PARK_L = 0, PARK_LI = 21, PARK_R = 27, PARK_J = 36, PARK_D = 45;
+constexpr int SCRATCH_EXCHANGE = 272;   // the default body's exchange area: Y^T [6][12] | vectors [4][12] | active [4] (+pad) | W' [12][12]
+constexpr int SCRATCH_FAST = SCRATCH_EXCHANGE + 4 * PARK + 8;
+static_assert(SCRATCH_FAST % 32 == 4 || SCRATCH_FAST % 32 == 12 || SCRATCH_FAST % 32 == 20 || SCRATCH_FAST % 32 == 28, "bank spread");
 // elements of T in one robot's shared scratch.  Its size and the offsets of its areas are multiples of 4 elements, so the P4<T> loads and
 // stores of the exchange stay aligned in both precisions whenever the first robot's scratch is.
 B2Q_HD constexpr int scratch_floats(int feat) { return feat ? SCRATCH_FLOATS : SCRATCH_FAST; }
@@ -302,6 +313,12 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
   // --- kinematics in B
   LegKin<T> K; leg_kin(md, lm, s.q, K);
   const V3<T> a1 = mk<T>(1, 0, 0), a2 = K.a2;
+  // the foot's terrain lookup (the substep's one branch before the exchange, on the terrain kind) comes first: the contact rows below then
+  // share one basic block with the Schur reduction and the Cholesky chain, and the scheduler can interleave the two independent chains
+  V3<T> toe_w = s.pos + rot(R, K.toe), n_w;
+  T hgt = terrain_height(cf, toe_w.x, toe_w.y, n_w);
+  T dist = toe_w.z - hgt - md.foot_r;
+  bool act = dist < cf.margin;
   V3<T> cL[3]; S3<T> IL[3]; T mL[3];
   {
     const R3<T>* Rs[3] = {&K.R1, &K.R2, &K.R3m};
@@ -316,6 +333,7 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
       mL[i] = lm.m[i] * pr.mscale[i];
     }
   }
+  B2Q_MARK(cm, RC_PD_KIN);
   // --- velocities and bias accelerations (q'' = 0, base twist derivative = 0, gravity as -g fictitious accel)
   V3<T> w1 = wB + a1 * s.qd[0], w2 = w1 + a2 * s.qd[1], w3 = w2 + a2 * s.qd[2];
   V3<T> pdd0 = cross(wB, vB) - gB;
@@ -378,6 +396,7 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     for (int c = 0; c < 6; c++) FD[j][c] = m_fma(Fa[2][c], D[2][j], m_fma(Fa[1][c], D[1][j], Fa[0][c] * D[0][j]));
   }
 
+  B2Q_MARK(cm, RC_BIAS_INERTIA);
   // --- leg contribution C_k - (F D) F^T to the base Schur complement and rhs; reduce over the 4 legs (4-lane butterflies)
   T S[21], r6[6];
   {
@@ -439,11 +458,8 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
   V3<T> wBs = wB + nud.a * dt, vBs = vB + (nud.l + cross(wB, vB)) * dt;
   T qds[3] = {s.qd[0] + dt * qdd[0], s.qd[1] + dt * qdd[1], s.qd[2] + dt * qdd[2]};
 
+  B2Q_MARK(cm, RC_SCHUR_CHOL);
   // --- contact rows of this lane's foot
-  V3<T> toe_w = s.pos + rot(R, K.toe), n_w;
-  T hgt = terrain_height(cf, toe_w.x, toe_w.y, n_w);
-  T dist = toe_w.z - hgt - md.foot_r;
-  bool act = dist < cf.margin;
   V3<T> t1w = mk<T>(1 - n_w.x * n_w.x, -n_w.x * n_w.y, -n_w.x * n_w.z);
   t1w = t1w * m_rsqrt(dot(t1w, t1w));
   V3<T> t2w = cross(n_w, t1w);
@@ -476,6 +492,7 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
       for (int e2 = 0; e2 < 3; e2++) Wl[e2][e] = Jk[e2][0] * dj[0] + Jk[e2][1] * dj[1] + Jk[e2][2] * dj[2];
     }
   }
+  B2Q_MARK(cm, RC_CONTACT_ROWS);
   T lk[3] = {T(0), T(0), T(0)};   // this lane's own toe impulses
   // extra rows of this leg in the FEAT variant: knee contact (n, t1, t2) and the three joint-limit rows: impulses, base-space Y rows, joint-space Jacobians
   T lkx[6] = {T(0), T(0), T(0), T(0), T(0), T(0)}, Yx[6][6], Jx[6][3];
@@ -590,6 +607,17 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     T* vecs = sh + 72;     // [4][12]  1/W_ii (0 = inactive row) | unconstrained velocity | target velocity | warm start
     T* afs = sh + 120;     // [4]      foot active
     T* Wp = sh + 128;      // [12][12] Wp[r][i] = W'_ir
+    T* park = sh + SCRATCH_EXCHANGE + k;   // park[4 * i]: this lane's value i, read back after the sweep (no other lane touches it)
+#pragma unroll
+    for (int i = 0; i < 21; i++) park[4 * (PARK_L + i)] = S[i];
+#pragma unroll
+    for (int i = 0; i < 6; i++) park[4 * (PARK_LI + i)] = Li[i];
+    park[4 * (PARK_R + 0)] = R.cx.x; park[4 * (PARK_R + 1)] = R.cx.y; park[4 * (PARK_R + 2)] = R.cx.z; park[4 * (PARK_R + 3)] = R.cy.x; park[4 * (PARK_R + 4)] = R.cy.y;
+    park[4 * (PARK_R + 5)] = R.cy.z; park[4 * (PARK_R + 6)] = R.cz.x; park[4 * (PARK_R + 7)] = R.cz.y; park[4 * (PARK_R + 8)] = R.cz.z;
+#pragma unroll
+    for (int i = 0; i < 9; i++) park[4 * (PARK_J + i)] = Jk[i / 3][i % 3];
+    park[4 * (PARK_D + 0)] = D[0][0]; park[4 * (PARK_D + 1)] = D[0][1]; park[4 * (PARK_D + 2)] = D[0][2]; park[4 * (PARK_D + 3)] = D[1][1]; park[4 * (PARK_D + 4)] = D[1][2];
+    park[4 * (PARK_D + 5)] = D[2][2];
     const T targ_n = dist > T(0) ? -dist * idt : cf.erp * (-dist) * idt;
     T invo[3];
 #pragma unroll
@@ -597,7 +625,8 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
       T d = Wl[e][e];
 #pragma unroll
       for (int c = 0; c < 6; c++) d = m_fma(Y[e][c], Y[e][c], d);
-      invo[e] = act ? m_rcp(d) : T(0);
+      const T rd = m_rcp(d);   // unconditional, so that the select keeps the exchange in one basic block
+      invo[e] = act ? rd : T(0);
       const int i = 3 * k + e;
 #pragma unroll
       for (int c = 0; c < 6; c++) YT[c * 12 + i] = Y[e][c];
@@ -676,7 +705,7 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
     // (measured: alternating between two areas instead costs 10 % — more shared memory per CTA and parity-dependent addressing)
     cm.sync();
   }
-  B2Q_MARK(cm, RC_PRE_SWEEP);
+  B2Q_MARK(cm, RC_DELASSUS);
   // --- projected Gauss-Seidel, Bullet row order: normals of feet 0..3, then (t1,t2) of feet 0..3.
   //     Row update = clamp -> delta -> 11 independent scalar FFMAs (W'_rr = 0: the row's own candidate is unchanged).
   //     A sweep in which no lambda changes (every dl = 0) leaves g unchanged too, so every later sweep would repeat it exactly: the
@@ -713,6 +742,26 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
   B2Q_MARK(cm, RC_SWEEP);
 #pragma unroll
   for (int f = 0; f < 4; f++) if (f == k) { lk[0] = lam[3 * f]; lk[1] = lam[3 * f + 1]; lk[2] = lam[3 * f + 2]; }   // own impulses (no dynamic register indexing)
+  {
+    // the parked operands of the impulse application (the barrier before the sweep orders these loads after the stores)
+    const T* park = cm.template scratch<T>() + SCRATCH_EXCHANGE + k;
+#pragma unroll
+    for (int i = 0; i < 21; i++) S[i] = park[4 * (PARK_L + i)];
+#pragma unroll
+    for (int i = 0; i < 6; i++) Li[i] = park[4 * (PARK_LI + i)];
+    R.cx = mk<T>(park[4 * (PARK_R + 0)], park[4 * (PARK_R + 1)], park[4 * (PARK_R + 2)]); R.cy = mk<T>(park[4 * (PARK_R + 3)], park[4 * (PARK_R + 4)], park[4 * (PARK_R + 5)]);
+    R.cz = mk<T>(park[4 * (PARK_R + 6)], park[4 * (PARK_R + 7)], park[4 * (PARK_R + 8)]);
+#pragma unroll
+    for (int i = 0; i < 9; i++) Jk[i / 3][i % 3] = park[4 * (PARK_J + i)];
+    D[0][0] = park[4 * (PARK_D + 0)]; D[0][1] = D[1][0] = park[4 * (PARK_D + 1)]; D[0][2] = D[2][0] = park[4 * (PARK_D + 2)]; D[1][1] = park[4 * (PARK_D + 3)];
+    D[1][2] = D[2][1] = park[4 * (PARK_D + 4)]; D[2][2] = park[4 * (PARK_D + 5)];
+    const T* YT = cm.template scratch<T>();   // the lane's own three rows of Y^T, which only this lane writes
+#pragma unroll
+    for (int e = 0; e < 3; e++) {
+#pragma unroll
+      for (int c = 0; c < 6; c++) Y[e][c] = YT[c * 12 + 3 * k + e];
+    }
+  }
   }
   s.lam_n = lk[0]; s.contact = lk[0] > T(0); s.lam_lim[0] = lkx[3]; s.lam_lim[1] = lkx[4]; s.lam_lim[2] = lkx[5];
   // --- apply impulses: sum over feet of Y_f lam_f by a 4-lane butterfly of each lane's own rows (keeps the gathered rows
@@ -742,7 +791,8 @@ B2Q_HD void substep(const Comm& cm, const Cfg<T>& cf, const Model<T>& md, const 
   {
     T wx = s.vang.x, wy = s.vang.y, wz = s.vang.z, th = m_sqrt(wx * wx + wy * wy + wz * wz) * dt;
     T sh, cw; sincos_t(T(0.5) * th, sh, cw);
-    T kk = th < T(1e-4) ? T(0.5) - th * th * T(1.0 / 48.0) : sh * m_rcp(th);
+    const T rth = m_rcp(th);   // unconditional (a select, no branch); unused below th = 1e-4
+    T kk = th < T(1e-4) ? T(0.5) - th * th * T(1.0 / 48.0) : sh * rth;
     T dx = wx * dt * kk, dy = wy * dt * kk, dz = wz * dt * kk;
     T ox = cw * s.qx + dx * s.qw + dy * s.qz - dz * s.qy;
     T oy = cw * s.qy - dx * s.qz + dy * s.qw + dz * s.qx;

@@ -3,9 +3,10 @@
 Builds the library with -DB2Q_REGION_CLOCKS into its own path (never csrc/libb2q.so, whose step kernel has no clock reads), runs
 bench.py's flagship workload through it (4096 envs, flat terrain, the Opt_with_points(0.1, 0.05) ETG, uniform +-0.3 residuals,
 auto-reset, L2 flushed between steps) and reads back one row per warp: the cycles lane 0 spent in each region, summed over the timed
-steps.  Regions (b2q_sim.cuh, RC_*): prologue (model staging, state and parameter loads), per substep the dynamics and Delassus build
-before the PGS sweep, the sweep, the impulse application and integration after it, the loop between substeps (observation-ring
-writes), and the epilogue (ETG, observation, reward, auto-reset, stores).
+steps.  Regions (b2q_sim.cuh, RC_*): prologue (model staging, state and parameter loads); per substep, before the PGS sweep, PD and
+kinematics, bias forces and composite inertias, Schur reduction and Cholesky, contact rows and the Delassus exchange (reported together
+as pre_sweep too); the sweep, the impulse application and integration after it, the loop between substeps (observation-ring writes),
+and the epilogue (ETG, observation, reward, auto-reset, stores).
 
 These are INSTRUMENTED numbers: the clock reads cost a few cycles each and constrain the scheduling around them.  The step time users
 get is the one bench.py reports from the product library.
@@ -24,7 +25,9 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-REGIONS = ["prologue", "pre_sweep", "sweep", "post_sweep", "between_substeps", "epilogue"]   # RC_* order of b2q_sim.cuh
+REGIONS = ["prologue", "pd_kinematics", "bias_inertia", "schur_cholesky", "contact_rows", "delassus_exchange",
+           "sweep", "post_sweep", "between_substeps", "epilogue"]                              # RC_* order of b2q_sim.cuh
+PRE_SWEEP = REGIONS[1:6]                                                                     # the substep's part before the sweep
 COLS = len(REGIONS) + 2                                                                       # + entry-to-exit cycles, launches
 
 
@@ -100,8 +103,10 @@ def main():
     res = {"instrumented": True, "kernel": "b2q_step_kernel<float, 0>", "envs": n, "warps": warps, "steps": K, "warmup": W,
            "substeps": R, "sweeps_per_substep": iters, "rows_per_sweep": 12, "lib": lib_path,
            "card": card(), "clocks_during_timed_steps": clocks, "us_per_step_instrumented": us, "regions": {}}
-    for i, name in enumerate(REGIONS + ["total"]):
-        c = per_step[:, i]
+    cols = {name: per_step[:, i] for i, name in enumerate(REGIONS)}
+    cols["pre_sweep"] = sum(cols[name] for name in PRE_SWEEP)
+    cols["total"] = total
+    for name, c in cols.items():
         res["regions"][name] = {"median": float(np.median(c)), "max": float(c.max()), "share": float(c.sum() / total.sum())}
     sw = per_step[:, REGIONS.index("sweep")]
     res["sweep_cycles_per_sweep"] = {"median": float(np.median(sw)) / (R * iters), "max": float(sw.max()) / (R * iters)}
