@@ -1,4 +1,5 @@
-/* b2q_deploy.h — C ABI of the deployment-rehearsal kernels: the control law of the reference's deployment/test.py:93-99 on an env handle.
+/* b2q_deploy.h — C ABI of the deployment-rehearsal kernels: the control law of the reference's deployment/test.py:93-99 on an env handle,
+ * and its optional open-loop Bezier gait (--gait 1).
  *
  * Deployment does not run the in-kernel ETG generator.  Step i of an episode applies
  *     base + act_bound * student(obs) + table[i]                                   (test.py:95-99)
@@ -32,6 +33,26 @@ int b2q_deploy_obs(B2QHandle h, const void* table, int rows, int etg_col, int no
  * the student plus the table, without the base pose). */
 int b2q_deploy_act(B2QHandle h, const float* policy_out, double act_bound, const void* table, int rows, void* action, void* rec_act,
                    int rec_rows, void* stream);
+
+/* Open-loop Bezier gait (test.py --gait 1: GaitWrapper, EnvWrapper.py:123-193, with BezierGait of utilities/Bezier.py and the A1 IK).
+ * The gait's joint angles take the place of the base pose: step i applies IK(feet_i) + act_bound * student(obs) + table[i], i.e. on an
+ * etg_enabled = 0 handle the action gets IK(feet_i) - POSE_ORI added (POSE_ORI = [0, 0.9, -1.8] x 4).  The gait arithmetic is float64 in
+ * both precisions (csrc/b2q_bezier.h).  state: the caller's device buffer [N][B2Q_BEZIER_STATE_DIM] doubles, per env
+ *     [0..11] T_b0 (the feet at reset, legs 0..3 x (x, y, z), base frame)  [12] time  [13] TD_time  [14] time_since_last_TD  [15] SwRef
+ *     [16] TD (0/1)  [17] StanceSwing of the reference leg (0 stance, 1 swing)
+ * Both calls refuse a handle created with etg_enabled = 1. */
+#define B2Q_BEZIER_STATE_DIM 18
+
+/* GaitWrapper.reset: T_b0 = the A1 forward kinematics of each env's current joint angles (b2q_get_state columns 13..24); the clock and
+ * touchdown state are zeroed and StanceSwing is set to swing, as a fresh BezierGait.  Call it after b2q_reset. */
+int b2q_bezier_reset(B2QHandle h, void* state, void* stream);
+
+/* GaitWrapper.step before env.step: with r_e the env's step counter (timesteps = r_e + 1; the first five steps hold the reset feet) and
+ * the reference foot's contact bit obs[e][contact_col] == 1 (the FootContactSensor column of the observation the student saw), advances
+ * the gait, computes the four feet and their IK and adds (IK - POSE_ORI), rounded once to the handle's type, to action [N,12] in place.
+ * An unreachable foot gives NaN angles, so the step kernel's non-finite check ends that env's episode.  0 <= contact_col < obs_dim.
+ * rec_feet [rec_rows,4,3] double or NULL: env 0's feet are written to rec_feet[r_0] when r_0 < rec_rows. */
+int b2q_bezier_act(B2QHandle h, void* state, int contact_col, const void* obs, void* action, double* rec_feet, int rec_rows, void* stream);
 
 #ifdef __cplusplus
 }

@@ -83,6 +83,8 @@ SYMBOLS = {
     # deployment rehearsal — include/b2q_deploy.h
     "b2q_deploy_obs": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp]),
     "b2q_deploy_act": (_i, [_vp, _vp, C.c_double, _vp, _i, _vp, _vp, _i, _vp]),
+    "b2q_bezier_reset": (_i, [_vp, _vp, _vp]),
+    "b2q_bezier_act": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp]),
 }
 
 

@@ -523,7 +523,8 @@ struct EnvT : EnvBase {
     return B2Q_OK;
   }
   void view(EnvView* v) const override {
-    v->N = B.N; v->obs_dim = obs_dim; v->elem_size = (int)sizeof(T); v->device = cfg.device; v->step_count = B.step_count; v->model = d_model;
+    v->N = B.N; v->obs_dim = obs_dim; v->elem_size = (int)sizeof(T); v->device = cfg.device; v->etg_enabled = cfg.etg_enabled;
+    v->step_count = B.step_count; v->model = d_model; v->state = B.state;
   }
   int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
              int32_t* seg, cudaStream_t s) override {

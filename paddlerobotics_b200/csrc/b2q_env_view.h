@@ -7,9 +7,10 @@
 namespace b2q {
 
 struct EnvView {
-  int N, obs_dim, elem_size, device;
+  int N, obs_dim, elem_size, device, etg_enabled;
   const int32_t* step_count;   // [N] device: control steps since each env's reset (the step kernel's B.step_count)
   const void* model;           // device Model<T> (T = float for elem_size 4, double for 8)
+  const void* state;           // device P4<T> state packs [NS][N]; packs 4..7 hold the joint angles of legs 0..3 in x, y, z
 };
 
 // B2Q_EINVAL for a NULL handle
