@@ -71,6 +71,26 @@ class BCReplayMemory:
     def sample_batch_by_index(self, idx):
         return self.obs[idx], self.ref_obs[idx]
 
+    def state_dict(self):
+        """The ring's rows up to the fill level and its cursor (position, fill level), as CPU tensors: a part-filled ring is not copied
+        whole."""
+        n = self._size
+        return {"max_size": self.max_size, "obs_dim": self.obs.shape[1], "ref_obs_dim": self.ref_obs.shape[1], "obs": self.obs[:n].cpu(),
+                "ref_obs": self.ref_obs[:n].cpu(), "pos": self._pos, "size": n}
+
+    def load_state_dict(self, sd):
+        """Restores a state_dict() into this memory's buffers (same capacity and widths); rows past the fill level are zeroed."""
+        have = (self.max_size, self.obs.shape[1], self.ref_obs.shape[1])
+        if (sd["max_size"], sd["obs_dim"], sd["ref_obs_dim"]) != have:
+            raise ValueError("BC replay memory state of shape %s, this memory is %s" % ((sd["max_size"], sd["obs_dim"], sd["ref_obs_dim"]), have))
+        n = int(sd["size"])
+        for k in ("obs", "ref_obs"):
+            buf = getattr(self, k)
+            buf[:n].copy_(sd[k])
+            buf[n:].zero_()
+        self._pos, self._size = int(sd["pos"]), n
+        torch.cuda.current_stream(self.obs.device).synchronize()     # the CPU sources must not be freed before the copies ran
+
     # ---- device path (b2q_bc_observe / b2q_bc_gather_cursor, include/b2q_rpm.h): float32 CUDA storage
     def observe(self, obs, step, noise=True, append=True, seed=0):
         """One control step in one launch: the student rows obs[:, 3:] + the sensor noise of BCtrain.py:53-59 (Philox key (seed, step),

@@ -12,6 +12,7 @@ batched loop at the control step that crosses it, over the first min(multiple, m
 reference's ring held at that multiple).  The learner work per collected row is the reference's.
 
     python -m paddlerobotics_b200.bctrain --ref_agent expert.pt --ETG_path expert.npz --num_envs 4096
+    python -m paddlerobotics_b200.bctrain --ref_agent expert.pt --ETG_path expert.npz --save_state 1; python -m paddlerobotics_b200.bctrain --resume BCtrain_log/exp0/state.pt --max_steps N
 """
 import argparse
 import json
@@ -85,7 +86,16 @@ def parser():
     p.add_argument("--render_dir", type=str, default="", help="--eval 1: write env 0's camera image of every step to DIR/img{step}.png")
     p.add_argument("--render_width", type=int, default=640)
     p.add_argument("--render_height", type=int, default=480)
+    p.add_argument("--save_state", type=int, default=0, help="1: write the whole training state (envs, student learner, BC ring, expert, gait, "
+                   "generators, counters) to <outdir>/<suffix>/state.pt after every evaluation block and when --max_steps is reached, replacing the "
+                   "previous file atomically")
+    p.add_argument("--resume", type=str, default="", help="a state.pt of bctrain --save_state: continue that run with its arguments (bit for bit until "
+                   "the first BC update, then as close as two uninterrupted runs: the learner sums with f32 atomics); only --max_steps, --outdir, "
+                   "--suffix and --save_state may be given with other values")
     return p
+
+
+RESUME_FREE = ("max_steps", "outdir", "suffix", "save_state", "resume")      # the flags a --resume may change
 
 
 def check_supported(args):
@@ -182,21 +192,36 @@ def run_episodes(env, policy, w, b, act_bound, max_step, x_noise=0, render=None)
 
 
 def main(argv=None):
-    args = parser().parse_args(argv)
+    from . import run_state
+    p = parser()
+    args = p.parse_args(argv)
+    state = None
+    if args.resume:
+        state = run_state.load_state(p, args.resume, "bctrain")
+        args = run_state.resume_args(p, parser, argv, state["args"], RESUME_FREE, (("--load", "load"), ("--ETG_path", "ETG_path"), ("--eval 1", "eval")),
+                                     "the student, the expert, the gait and the training loop")
+    if args.save_state and not args.outdir:
+        p.error("--save_state 1 writes <outdir>/<suffix>/state.pt: it needs --outdir")
     check_supported(args)
     torch.manual_seed(args.seed); np.random.seed(args.seed)
-    w, b = etg_of_path(args.ETG_path, args.ETG_T)
+    # a resume takes the gait and the expert from the state, not from --ETG_path / --ref_agent, whose files may have changed since
+    w, b = etg_of_path(args.ETG_path, args.ETG_T) if state is None else (state["w"], state["b"])
     bound = torch.as_tensor(act_bound_of(args), dtype=torch.float32, device="cuda")
     student = MujocoAgent(46, 12, seed=args.seed)
-    if args.load:
+    if args.load and state is None:
         student.restore(args.load)
     if args.eval:
         return evaluate(args, student, w, b, bound)
     n, memory, every = args.num_envs, int(args.memory), int(args.eval_every_steps)
     expert = MujocoAgent(49, 12, seed=args.seed)
-    expert.restore(args.ref_agent)
+    if state is None:
+        expert.restore(args.ref_agent)
+    else:
+        expert.load_state_dict(state["expert"])
     e_step = args.e_step
     env = make_vec_env(args, n, auto_reset=True, max_episode_steps=e_step + 1)
+    # The evaluation env needs no snapshot: random_eval resets every env of it before each episode, and neither it nor the student's
+    # evaluation noise (keyed by the step number) draws from a generator that lives across evaluations.
     eval_env = make_vec_env(args, args.eval_envs, auto_reset=False)
     learner = SACLearner(student, args.batch, actor_lr=ACTOR_LR, critic_lr=CRITIC_LR)
     rpm = bc.BCReplayMemory(memory, 46, 49, device=env.device)
@@ -208,6 +233,22 @@ def main(argv=None):
     total, it, updates, test_flag, t0 = 0, 0, 0, 0, time.perf_counter()
     ret_acc = torch.zeros(n, device=env.device); ep_sum = torch.zeros((), device=env.device); ep_cnt = torch.zeros((), device=env.device)
     log = []
+    run_args = dict(vars(args))                                                            # what a --save_state file records
+    if state is not None:
+        # the learner's bc_sweep graphs are captured again at its first sweep: a new learner holds none
+        env.load_state_dict(state["env"]); learner.load_state_dict(state["learner"]); rpm.load_state_dict(state["rpm"])
+        gen.set_state(state["gen"]); np.random.set_state(state["np_random"])
+        obs.copy_(state["obs"]); ret_acc.copy_(state["ret_acc"]); ep_sum.copy_(state["ep_sum"]); ep_cnt.copy_(state["ep_cnt"])
+        total, it, updates, test_flag, e_step = (state["loop"][k] for k in ("total", "it", "updates", "test_flag", "e_step"))
+        torch.cuda.synchronize()                                                           # the CPU sources are freed on return
+
+    def save_state():
+        torch.cuda.synchronize()
+        run_state.write_atomic(os.path.join(outdir, "state.pt"), {
+            "command": "bctrain", "args": run_args, "env": env.state_dict(), "learner": learner.state_dict(), "rpm": rpm.state_dict(),
+            "expert": expert.state_dict(), "w": np.array(w), "b": np.array(b), "gen": gen.get_state(), "np_random": np.random.get_state(),
+            "obs": obs.cpu(), "ret_acc": ret_acc.cpu(), "ep_sum": ep_sum.cpu(), "ep_cnt": ep_cnt.cpu(),
+            "loop": {"total": total, "it": it, "updates": updates, "test_flag": test_flag, "e_step": e_step}})
     while total < args.max_steps:
         warm = rpm.size() < args.warmup                                                       # BCtrain.py:102-105
         a_obs = rpm.observe(obs, it, noise=noise, append=True, seed=args.seed)             # BCtrain.py:98-99,120
@@ -246,6 +287,10 @@ def main(argv=None):
                 env.set_max_episode_steps(e_step + 1)
             learner.pull()
             student.save(os.path.join(outdir, "itr_%d.pt" % total))
+            if args.save_state:
+                save_state()
+    if args.save_state:
+        save_state()
     torch.cuda.synchronize()
     learner.pull()
     env.close(); eval_env.close()

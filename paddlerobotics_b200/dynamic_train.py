@@ -15,6 +15,7 @@ global RNG, which the reference leaves unseeded.  In training, --load does not s
 starts from zeros.  --alg cma is refused: the reference's set_solver has no cma branch.
 
     python -m paddlerobotics_b200.dynamic_train --data_dir data/dynamic --alg ga --steps 10000
+    python -m paddlerobotics_b200.dynamic_train --data_dir data/dynamic --save_state 1; python -m paddlerobotics_b200.dynamic_train --resume Dynamic/exp0/state.pt --steps N
     python -m paddlerobotics_b200.dynamic_train --eval 1 --load Dynamic/exp0/dynamic_param9027.npy
     python -m paddlerobotics_b200.train --dynamic_param Dynamic/exp0/dynamic_param9027.npy     # train the expert on the result
 """
@@ -52,7 +53,14 @@ def parser():
     # ---- the data the reference reads from fixed paths, and its RNG
     p.add_argument("--data_dir", type=str, default="data/dynamic", help="holds %s" % ", ".join(DATA_FILES.values()))
     p.add_argument("--seed", type=int, default=0, help="seeds np.random before the solver is built: every rank asks the same population")
+    p.add_argument("--save_state", type=int, default=0, help="1: rank 0 writes the solver and the next epoch to <outdir>/<suffix>/state.pt after every "
+                   "epoch with a height evaluation and after the last epoch, replacing the previous file atomically")
+    p.add_argument("--resume", type=str, default="", help="a state.pt of dynamic_train --save_state: continue that search bit for bit with its arguments "
+                   "(every rank loads it); only --steps, --outdir, --suffix and --save_state may be given with other values")
     return p
+
+
+RESUME_FREE = ("steps", "outdir", "suffix", "save_state", "resume")      # the flags a --resume may change
 
 
 def make_solver(alg, popsize, sigma, num_params=NUM_PARAMS, sigma_decay=SIGMA_DECAY):
@@ -108,8 +116,15 @@ def load_data(data_dir):
 
 
 def main(argv=None):
+    from . import run_state
     p = parser()
     args = p.parse_args(argv)
+    state = None
+    if args.resume:
+        state = run_state.load_state(p, args.resume, "dynamic_train")
+        args = run_state.resume_args(p, parser, argv, state["args"], RESUME_FREE, (("--load", "load"), ("--eval 1", "eval")), "the solver and the epoch")
+    if args.save_state and not args.outdir:
+        p.error("--save_state 1 writes <outdir>/<suffix>/state.pt: it needs --outdir")
     if args.alg not in ALGS:
         p.error("--alg %s is not provided (the reference's set_solver has no %s branch); supported algorithms: %s" % (args.alg, args.alg, ", ".join(ALGS)))
     if args.eval and not args.load:
@@ -129,14 +144,17 @@ def main(argv=None):
     if own_group:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     try:
-        return run(args, gait, mean_dict, rank, world, local)
+        return run(args, gait, mean_dict, rank, world, local, state)
     finally:
         if own_group:
             dist.destroy_process_group()
 
 
-def run(args, gait, mean_dict, rank, world, local):
-    """The epochs (or the --eval evaluation) on this rank; returns the records rank 0 printed."""
+def run(args, gait, mean_dict, rank, world, local, state=None):
+    """The epochs (or the --eval evaluation) on this rank; returns the records rank 0 printed.  `state`: a --save_state file to continue
+    from (its solver, NumPy's RNG included, and its next epoch).  The evaluators set every env's dynamics and reset it before each
+    replay, so they carry nothing between epochs and need no snapshot."""
+    from . import run_state
     from .es import DynamicsEvaluator
     popsize = args.K * args.thread
     cfg = evaluator_config()
@@ -154,11 +172,16 @@ def run(args, gait, mean_dict, rank, world, local):
         return [rec]
     np.random.seed(args.seed)
     solver = make_solver(args.alg, popsize, args.sigma)
+    start = 0
+    if state is not None:
+        solver.load_state_dict(state["solver"])
+        start = int(state["epoch"])
     evaluator = DynamicsEvaluator(popsize, gait, mean_dict, keys=("exp", "ori"), steps=STEPS, rank=rank, world=world, device=local, **cfg)
     outdir = os.path.join(args.outdir, args.suffix)
     if rank == 0:
         os.makedirs(outdir, exist_ok=True)
-    for epoch in range(args.steps):                                          # ES_ParallelModel.update / train, :152-190
+    run_args = dict(vars(args))                                              # what a --save_state file records
+    for epoch in range(start, args.steps):                                   # ES_ParallelModel.update / train, :152-190
         solutions = solver.ask()
         rewards = evaluator.evaluate(solutions).double().cpu().numpy()
         solver.tell(rewards)
@@ -171,6 +194,9 @@ def run(args, gait, mean_dict, rank, world, local):
             if epoch % 5 == 0 and epoch > 0:
                 rec = {"epoch": epoch, "eval_reward": eval_height(result[0])}
                 log.append(rec); print(json.dumps(rec), flush=True)
+            if args.save_state and ((epoch % 5 == 0 and epoch > 0) or epoch == args.steps - 1):
+                run_state.write_atomic(os.path.join(outdir, "state.pt"), {"command": "dynamic_train", "args": run_args, "solver": solver.state_dict(),
+                                                                          "epoch": epoch + 1})
     evaluator.env.close()
     if height is not None:
         height.env.close()

@@ -22,7 +22,32 @@ def compute_weight_decay(weight_decay, model_param_list):
     return -weight_decay * np.mean(grid * grid, axis=1)
 
 
-class SimpleGA:
+class SolverState:
+    """state_dict() / load_state_dict() of the ES solvers (SimpleGA, PEPG, OpenES, SimpleES): every attribute, the Adam optimiser of
+    OpenES / PEPG among them, and NumPy's global RNG state, which ask() draws from."""
+
+    def state_dict(self):
+        """{"attrs": the attributes but the optimisers, "adam": {name: an optimiser's attributes but its solver}, "np_random"}.  One deep
+        copy of both, so arrays that alias each other (PEPG's best_mu can be mu itself) still do after a load."""
+        attrs = {k: v for k, v in vars(self).items() if not isinstance(v, Adam)}
+        adam = {k: {a: x for a, x in vars(v).items() if a != "pi"} for k, v in vars(self).items() if isinstance(v, Adam)}
+        attrs, adam = copy.deepcopy((attrs, adam))
+        return {"attrs": attrs, "adam": adam, "np_random": np.random.get_state()}
+
+    def load_state_dict(self, sd):
+        """Restores a state_dict(), NumPy's global RNG state included: the next ask() equals the saved solver's.  Each optimiser is rebuilt
+        on this solver (Adam.update moves this solver's mu)."""
+        attrs, adam = copy.deepcopy((sd["attrs"], sd.get("adam", {})))
+        self.__dict__.update(attrs)
+        for k, v in adam.items():
+            opt = Adam.__new__(Adam)
+            opt.__dict__.update(v)
+            opt.pi = self
+            setattr(self, k, opt)
+        np.random.set_state(sd["np_random"])
+
+
+class SimpleGA(SolverState):
     """Elitist GA with Gaussian mutation; same constructor/ask/tell/reset semantics as the reference class."""
 
     def __init__(self, num_params, sigma_init=0.1, sigma_decay=0.999, sigma_limit=0.01, popsize=256, elite_ratio=0.1,
@@ -39,15 +64,6 @@ class SimpleGA:
         self.best_reward = 0
         self.first_iteration = True
         self.forget_best, self.weight_decay = forget_best, weight_decay
-
-    def state_dict(self):
-        """The solver's attributes (sigma, elite set, best parameters, ...) and NumPy's global RNG state, which ask() draws from."""
-        return {"attrs": copy.deepcopy(vars(self)), "np_random": np.random.get_state()}
-
-    def load_state_dict(self, sd):
-        """Restores a state_dict(), NumPy's global RNG state included: the next ask() equals the saved solver's."""
-        self.__dict__.update(copy.deepcopy(sd["attrs"]))
-        np.random.set_state(sd["np_random"])
 
     def reset(self, param):
         self.best_param = np.copy(param)
@@ -139,7 +155,7 @@ class Adam:
         self.pi.mu = self.pi.mu + (-a * self.m / (np.sqrt(self.v) + self.epsilon))
 
 
-class SimpleES:
+class SimpleES(SolverState):
     """Gaussian search around mu; tell() moves mu to the softmax(3·normalised reward)-weighted mean of the population."""
 
     def __init__(self, num_params, popsize=256, sigma_init=0.1, sigma_decay=0.999, sigma_limit=0.01, weight_decay=0.01, param=None):
@@ -180,7 +196,7 @@ class SimpleES:
         return (self.best_mu, self.best_reward, self.curr_best_reward, self.sigma)
 
 
-class OpenES:
+class OpenES(SolverState):
     """OpenAI-ES: a Gaussian population around mu and a normalised-reward gradient step on mu."""
 
     def __init__(self, num_params, sigma_init=0.1, sigma_decay=0.999, sigma_limit=0.01, learning_rate=0.01, learning_rate_decay=0.9999,
@@ -235,7 +251,7 @@ class OpenES:
         return (self.best_mu, self.best_reward, self.curr_best_reward, self.sigma)
 
 
-class PEPG:
+class PEPG(SolverState):
     """Parameter-exploring policy gradients: antithetic pairs mu ± eps with a per-parameter sigma that adapts, each step clipped to
     ±sigma_max_change·sigma; with elite_ratio > 0, mu moves by the mean offset of the elite instead of the Adam step."""
 

@@ -18,6 +18,7 @@ never-updated ETG_best_param); a round that crosses several multiples evaluates 
 calls an agent that does not exist).  --epsilon, --gamma, --random and --e_step are accepted and ignored, as in the reference.
 
     python -m paddlerobotics_b200.pretrain --task_mode stairstair --popsize 40 --outdir pretrain_log
+    python -m paddlerobotics_b200.pretrain --outdir pretrain_log --save_state 1; python -m paddlerobotics_b200.pretrain --resume pretrain_log/exp0/state.pt --max_steps N
     python -m paddlerobotics_b200.pretrain --eval 1 --load pretrain_log/exp0/itr_160400.npz --render_dir frames
     python -m paddlerobotics_b200.train --task_mode stairstair --ETG_path pretrain_log/exp0/itr_160400.npz
 """
@@ -85,7 +86,14 @@ def parser():
     p.add_argument("--render_dir", type=str, default="", help="--eval 1: write env 0's camera image of every step to DIR/img{step}.png")
     p.add_argument("--render_width", type=int, default=640)
     p.add_argument("--render_height", type=int, default=480)
+    p.add_argument("--save_state", type=int, default=0, help="1: write the whole search state to <outdir>/<suffix>/state.pt after every evaluation block "
+                   "and when --max_steps is reached, replacing the previous file atomically")
+    p.add_argument("--resume", type=str, default="", help="a state.pt of pretrain --save_state: continue that search bit for bit with its arguments; "
+                   "only --max_steps, --outdir, --suffix and --save_state may be given with other values")
     return p
+
+
+RESUME_FREE = ("max_steps", "outdir", "suffix", "save_state", "resume")      # the flags a --resume may change
 
 
 def check_supported(args):
@@ -139,8 +147,16 @@ def checkpoint_names(round_totals, every):
 
 
 def main(argv=None):
+    from . import run_state
     p = parser()
     args = p.parse_args(argv)
+    state = None
+    if args.resume:
+        state = run_state.load_state(p, args.resume, "pretrain")
+        args = run_state.resume_args(p, parser, argv, state["args"], RESUME_FREE, (("--load", "load"), ("--ETG_path", "ETG_path"), ("--eval 1", "eval")),
+                                     "the solver, the incumbent and the search loop")
+    if args.save_state and not args.outdir:
+        p.error("--save_state 1 writes <outdir>/<suffix>/state.pt: it needs --outdir")
     check_supported(args)
     if args.eval and not args.load:
         p.error("--eval 1 evaluates a gait: it needs --load X.npz")
@@ -150,7 +166,7 @@ def main(argv=None):
         p.error("--popsize %d: SimpleGA's elite_ratio 0.1 needs a population of at least 10 to keep one parent" % args.popsize)
     if args.eval:
         return evaluate(args)
-    return pretrain(args)
+    return pretrain(args) if state is None else pretrain(args, state)
 
 
 def make_eval_env(args, cfg):
@@ -172,15 +188,20 @@ def evaluate(args):
     return rec
 
 
-def pretrain(args):
+def pretrain(args, state=None):
+    """The search; `state`: a --save_state file to continue from (its solver, incumbent and counters replace the set-up)."""
     import torch
+    from . import run_state
     from .env import apply_dynamic_param
     from .es import PopulationEvaluator, SimpleGA, solutions_to_etg_device
     from .etg import Opt_with_points
     from .train import EVAL_TERMS, etg_prior, initial_etg, run_evaluate_episodes
     np.random.seed(args.seed); torch.manual_seed(args.seed)
     layer, w0, b0, prior_points = etg_prior(args.ETG_T, args.footheight, args.steplen)
-    init, w_inc, b_inc = initial_etg(args)                                                                      # pretrain.py:171-177
+    if state is None:
+        init, w_inc, b_inc = initial_etg(args)                                                                  # pretrain.py:171-177
+    else:
+        init = np.zeros(12)                              # the saved solver replaces it: a resume does not read --ETG_path again
     solver = SimpleGA(12, sigma_init=args.sigma, sigma_decay=args.sigma_decay, sigma_limit=0.005, elite_ratio=0.1, weight_decay=0.005,
                       popsize=args.popsize, param=init.copy())                                                  # pretrain.py:178-185
     cfg = env_config(args)
@@ -198,10 +219,24 @@ def pretrain(args):
 
     # the incumbent seeds best_param / best_reward (the train.py:395-396 rule; both are undefined in the reference).  This evaluation is set-up:
     # env_steps counts the steps of the generations' rollouts only, so --max_steps bounds the search as the reference's total_steps would
-    inc = rollout(np.repeat(np.asarray(w_inc)[None], pop, 0), np.repeat(np.asarray(b_inc)[None], pop, 0))[0]
-    best_reward = float(np.nanmean(inc)) if np.isfinite(inc).any() else -np.inf
-    best_param = init.copy()
-    log, test_flag, es_step, env_steps = [], 0, 0, 0
+    # A resume skips it: best_reward is in the state.  Every rollout and evaluation resets all envs of its handle and draws no random numbers,
+    # so the envs carry nothing from one generation to the next and need no snapshot.
+    if state is None:
+        inc = rollout(np.repeat(np.asarray(w_inc)[None], pop, 0), np.repeat(np.asarray(b_inc)[None], pop, 0))[0]
+        best_reward = float(np.nanmean(inc)) if np.isfinite(inc).any() else -np.inf
+        best_param = init.copy()
+        test_flag, es_step, env_steps = 0, 0, 0
+    else:
+        solver.load_state_dict(state["solver"])
+        best_param, best_reward = np.array(state["best_param"]), state["best_reward"]
+        test_flag, es_step, env_steps = (state["loop"][k] for k in ("test_flag", "es_step", "env_steps"))
+    log = []
+    run_args = dict(vars(args))                          # what a --save_state file records
+
+    def save_state():
+        run_state.write_atomic(os.path.join(outdir, "state.pt"), {
+            "command": "pretrain", "args": run_args, "solver": solver.state_dict(), "best_param": np.array(best_param), "best_reward": best_reward,
+            "loop": {"test_flag": test_flag, "es_step": es_step, "env_steps": env_steps}})
     while env_steps < args.max_steps:
         for _ in range(args.es_train_steps):                                                                   # pretrain.py:221-256
             sol = solver.ask()
@@ -231,6 +266,10 @@ def pretrain(args):
             rec = {"env_steps": env_steps, "eval_return": r["mean_return"], "eval_length": r["mean_length"], "eval_success_rate": r["success_rate"],
                    "terms": r["terms"], "best_reward": best_reward, "checkpoint": os.path.basename(path)}
             log.append(rec); print(json.dumps(rec), flush=True)
+            if args.save_state:
+                save_state()
+    if args.save_state:
+        save_state()
     evaluator.env.close(); eval_env.close()
     return log
 

@@ -19,12 +19,13 @@ import time
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, run_state
 from .agent import MujocoAgent, SACLearner
 from .env import VecQuadrupedalEnv, apply_dynamic_param
 from .es import PopulationEvaluator, SimpleGA, TrainEpisodeStats, solutions_to_etg_device
 from .etg import ETG_layer, Opt_with_points
 from .replay import ReplayMemory
+from .run_state import write_atomic
 from .terrain import make_terrain
 
 GAMMA, TAU, ALPHA, ACTOR_LR, CRITIC_LR = 0.99, 0.005, 0.2, 3e-4, 3e-4     # train.py:43-47
@@ -150,44 +151,14 @@ def check_args(p, args):
 
 
 RESUME_FREE = ("max_steps", "log_every", "outdir", "suffix", "save_state", "resume")     # the flags a --resume may change
+RESUME_CONFLICTS = (("--load", "load"), ("--ETG_path", "ETG_path"), ("--eval 1", "eval"))
 
 
 def resume_args(p, argv, saved):
     """The arguments of a --resume run: the saved run's, with the RESUME_FREE flags of this command line.  Any other flag given on the
     command line with a value other than the saved one is an argument error (p.error) naming the flags, as are --load, --ETG_path and
     --eval 1, which set what the state restores."""
-    q = parser()
-    for a in q._actions:
-        a.default = argparse.SUPPRESS
-    given = vars(q.parse_args(argv))
-    conflicts = [f for f, bad in (("--load", given.get("load", "")), ("--ETG_path", given.get("ETG_path", "None") not in ("", "None")),
-                                  ("--eval 1", given.get("eval", 0))) if bad]
-    if conflicts:
-        p.error("--resume restores the agent, the ETG and the training loop: it cannot be combined with %s" % ", ".join(conflicts))
-    differ = sorted(k for k, v in given.items() if k not in RESUME_FREE and v != saved.get(k))
-    if differ:
-        p.error("--resume %s: these arguments differ from the saved run's: %s" % (given["resume"], ", ".join("--" + k for k in differ)))
-    args = argparse.Namespace(**saved)
-    for k in RESUME_FREE:
-        if k in given:
-            setattr(args, k, given[k])
-    return args
-
-
-def write_atomic(path, obj):
-    """torch.save(obj) to path through a temporary file that is flushed, fsynced and renamed over it: a crash mid-write leaves the
-    previous file intact."""
-    tmp = path + ".tmp"
-    with open(tmp, "wb") as f:
-        torch.save(obj, f)
-        f.flush()
-        os.fsync(f.fileno())
-    os.replace(tmp, path)
-    fd = os.open(os.path.dirname(os.path.abspath(path)), os.O_RDONLY)
-    try:
-        os.fsync(fd)                                                        # the rename itself
-    finally:
-        os.close(fd)
+    return run_state.resume_args(p, parser, argv, saved, RESUME_FREE, RESUME_CONFLICTS, "the agent, the ETG and the training loop")
 
 
 def grow_e_step(e_step, growth):
@@ -278,7 +249,7 @@ def main(argv=None):
     args = p.parse_args(argv)
     state = None
     if args.resume:
-        state = torch.load(args.resume, map_location="cpu", weights_only=False)
+        state = run_state.load_state(p, args.resume, "train")
         args = resume_args(p, argv, state["args"])
     if args.save_state and not args.outdir:
         p.error("--save_state 1 writes <outdir>/<suffix>/state.pt: it needs --outdir")
