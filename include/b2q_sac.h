@@ -66,6 +66,9 @@ int64_t b2q_sac_launch_count(B2QSacHandle h);
  * (b2q_sac_last_error names the field), then copies the buffers and rebuilds the bf16 tensor-core operand images with the packer
  * of b2q_sac_set_params, so the next learn is bit-identical to the saved learner's. */
 int64_t b2q_sac_snapshot_bytes(B2QSacHandle h);
+/* Byte offset in the snapshot of the loss buffer (4 floats: this learner's last losses, the one part that data-parallel ranks do not
+ * share); -1 for a NULL handle. */
+int64_t b2q_sac_snapshot_loss_offset(B2QSacHandle h);
 int b2q_sac_snapshot_save(B2QSacHandle h, void* dst, void* stream);
 int b2q_sac_snapshot_load(B2QSacHandle h, const void* src, void* stream);
 #ifdef __cplusplus

@@ -60,6 +60,7 @@ SYMBOLS = {
     "b2q_sac_loss_ptr": (_vp, [_vp]),
     "b2q_sac_launch_count": (C.c_int64, [_vp]),
     "b2q_sac_snapshot_bytes": (C.c_int64, [_vp]),
+    "b2q_sac_snapshot_loss_offset": (C.c_int64, [_vp]),
     "b2q_sac_snapshot_save": (_i, [_vp, _vp, _vp]),
     "b2q_sac_snapshot_load": (_i, [_vp, _vp, _vp]),
     # ES population fitness — include/b2q_es.h

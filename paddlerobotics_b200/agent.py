@@ -214,12 +214,14 @@ class SACLearner:
     """SAC.learn on the device (csrc/b2q_sac.cu): same hyper-parameters and update order as ETGRL/alg/sac.py:30-118.
     `world`>1: data-parallel learner, gradient buckets all-reduced (NCCL) between the gradient and optimiser phases."""
 
-    def __init__(self, agent, batch, gamma=0.99, tau=0.005, alpha=0.2, actor_lr=3e-4, critic_lr=3e-4, world=1, sync="exact"):
+    def __init__(self, agent, batch, gamma=0.99, tau=0.005, alpha=0.2, actor_lr=3e-4, critic_lr=3e-4, world=1, sync="exact", seed_key=0):
         """sync (world > 1): "exact" = the reference's update order (critic step, then the actor gradient against the UPDATED critic,
         sac.py:77-118) which needs two all-reduces; "flat" = both gradients against the pre-update parameters and ONE all-reduce of the
-        single flat bucket [actor | critic] (SURVEY §8e).  sync="flat" with world == 1 runs the same phase order on one GPU."""
+        single flat bucket [actor | critic] (SURVEY §8e).  sync="flat" with world == 1 runs the same phase order on one GPU.
+        seed_key: added to the step seed of the phase-by-phase learn() (the path of world > 1), so data-parallel ranks draw different rsample() noise for
+        their shards (train passes rank << 40: no step count reaches it); 0 keeps the single-GPU key."""
         self.lib = _lib.load()
-        self.agent, self.batch, self.world, self.sync = agent, batch, world, sync
+        self.agent, self.batch, self.world, self.sync, self.seed_key = agent, batch, world, sync, int(seed_key)
         self.allreduce_events = None
         self.h = C.c_void_p()
         rc = self.lib.b2q_sac_create(agent.device.index or 0, agent.obs_dim, agent.act_dim, batch, gamma, tau, alpha, actor_lr, critic_lr, C.byref(self.h))
@@ -263,14 +265,26 @@ class SACLearner:
         # wrap the device bucket without copying (for in-place NCCL all-reduce)
         return torch.as_tensor(_CudaBuf(self.lib.b2q_sac_grad_ptr(self.h, which), n), device=self.agent.device)
 
-    def state_dict(self):
-        """The learner's whole training state as CPU tensors: b2q_sac_snapshot_save (parameters, target, Adam moments, loss buffer, device
-        step counter) and the host step count, which seeds the eager learn() and a captured one."""
+    def _snapshot(self):
+        """b2q_sac_snapshot_save into a new device byte tensor."""
         blob = torch.empty(int(self.lib.b2q_sac_snapshot_bytes(self.h)), dtype=torch.uint8, device=self.agent.device)
         rc = self.lib.b2q_sac_snapshot_save(self.h, blob.data_ptr(), self._stream())
         if rc != 0:
             raise RuntimeError("b2q_sac_snapshot_save: %d %s" % (rc, self.lib.b2q_sac_last_error(self.h).decode()))
-        return {"snapshot": blob.cpu(), "steps": self.steps}
+        return blob
+
+    def state_dict(self):
+        """The learner's whole training state as CPU tensors: b2q_sac_snapshot_save (parameters, target, Adam moments, loss buffer, device
+        step counter) and the host step count, which seeds the eager learn() and a captured one."""
+        return {"snapshot": self._snapshot().cpu(), "steps": self.steps}
+
+    def replica_state(self):
+        """The part of the learner that data-parallel ranks keep identical, as one device byte tensor: the snapshot (parameters, target,
+        Adam moments, device step counter) with its loss buffer, which holds this rank's shard losses, zeroed."""
+        blob = self._snapshot()
+        off = int(self.lib.b2q_sac_snapshot_loss_offset(self.h))
+        blob[off:off + 4 * 4].zero_()                                   # the loss buffer: 4 floats
+        return blob
 
     def load_state_dict(self, sd):
         """Restores a state_dict() of a learner with the same shapes and hyper-parameters, then pull()s the weights into the agent."""
@@ -307,7 +321,7 @@ class SACLearner:
         eps_cur = None if eps_cur is None else t(eps_cur)
         pe = lambda x: None if x is None else x.data_ptr()
         self.steps += 1
-        args = (obs.data_ptr(), act.data_ptr(), rew.data_ptr(), next_obs.data_ptr(), term.data_ptr(), pe(eps_next), pe(eps_cur), C.c_uint64(self.steps))
+        args = (obs.data_ptr(), act.data_ptr(), rew.data_ptr(), next_obs.data_ptr(), term.data_ptr(), pe(eps_next), pe(eps_cur), C.c_uint64(self.steps + self.seed_key))
         if self.world == 1 and graph:
             # one learner step replayed from a CUDA graph (static input buffers; inputs that already ARE the static buffers are not copied)
             ins = [obs, act, rew, next_obs, term]

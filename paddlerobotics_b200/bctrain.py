@@ -195,6 +195,9 @@ def main(argv=None):
     from . import run_state
     p = parser()
     args = p.parse_args(argv)
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise NotImplementedError("bctrain under torchrun (WORLD_SIZE %s): its BC update has no data-parallel path; run it on one GPU"
+                                  % os.environ["WORLD_SIZE"])
     state = None
     if args.resume:
         state = run_state.load_state(p, args.resume, "bctrain")

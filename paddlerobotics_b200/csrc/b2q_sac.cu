@@ -787,6 +787,13 @@ float* b2q_sac_grad_ptr(B2QSacHandle s, int which) { return !s ? nullptr : (whic
 float* b2q_sac_loss_ptr(B2QSacHandle s) { return s ? s->losses : nullptr; }
 
 int64_t b2q_sac_snapshot_bytes(B2QSacHandle s) { return s ? sac_snapshot_bytes(s) : -1; }
+int64_t b2q_sac_snapshot_loss_offset(B2QSacHandle s) {
+  if (!s) return -1;
+  SacPart parts[8]; sac_parts(s, parts);
+  int64_t off = (int64_t)b2q_snap::HDR_BYTES;
+  for (int i = 0; parts[i].p != s->losses; i++) off += (int64_t)(parts[i].n * sizeof(float));
+  return off;
+}
 int b2q_sac_snapshot_save(B2QSacHandle s, void* dst, void* stream) {
   if (!s) return -1;
   if (!dst || ((size_t)dst & 15)) { s->err = "b2q_sac_snapshot_save: dst must be a 16-byte aligned device pointer"; return -1; }

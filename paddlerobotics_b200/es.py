@@ -465,11 +465,15 @@ class TrainEpisodeStats:
     def load_state_dict(self, sd):
         self.run.copy_(sd["run"]); self.win.copy_(sd["win"])
 
-    def take(self):
+    def take(self, reduce=None):
         """The window's means over its finite episodes, then an empty window.  {episodes, nonfinite_episodes, return, length, terms: {term:
-        mean episode sum}, mean_terms: {term: mean of sum / length}, success_rate}; the means are None when no finite episode closed."""
+        mean episode sum}, mean_terms: {term: mean of sum / length}, success_rate}; the means are None when no finite episode closed.
+        reduce(sums): applied in place to the window sums [5 + 2 nt] before the means, e.g. a sum over the ranks of a sharded run."""
         nt = len(self.terms)
-        s = self.win.sum(1).tolist()
+        s = self.win.sum(1)
+        if reduce is not None:
+            reduce(s)
+        s = s.tolist()
         self.win.zero_()
         k = s[0]
         m = (lambda x: x / k) if k > 0 else (lambda x: None)

@@ -21,6 +21,12 @@ calls an agent that does not exist).  --epsilon, --gamma, --random and --e_step 
     python -m paddlerobotics_b200.pretrain --outdir pretrain_log --save_state 1; python -m paddlerobotics_b200.pretrain --resume pretrain_log/exp0/state.pt --max_steps N
     python -m paddlerobotics_b200.pretrain --eval 1 --load pretrain_log/exp0/itr_160400.npz --render_dir frames
     python -m paddlerobotics_b200.train --task_mode stairstair --ETG_path pretrain_log/exp0/itr_160400.npz
+    torchrun --nproc_per_node 8 -m paddlerobotics_b200.pretrain --popsize 256 --es_rollouts 16 --outdir pretrain_log
+
+Under torchrun (WORLD_SIZE > 1) every rank seeds NumPy alike and asks the same population; it rolls out its contiguous shard of the
+individuals, and one all-gather per generation (fitness, length, term sums and success rate) gives every rank the whole table, so every
+rank tells the same fitness and the run computes what one GPU computes with the same --popsize and --es_rollouts.  --popsize must be
+divisible by the ranks.  Rank 0 alone evaluates, prints and writes itr_*.npz and state.pt; a --resume loads the file on every rank.
 """
 import argparse
 import json
@@ -89,11 +95,13 @@ def parser():
     p.add_argument("--save_state", type=int, default=0, help="1: write the whole search state to <outdir>/<suffix>/state.pt after every evaluation block "
                    "and when --max_steps is reached, replacing the previous file atomically")
     p.add_argument("--resume", type=str, default="", help="a state.pt of pretrain --save_state: continue that search bit for bit with its arguments; "
-                   "only --max_steps, --outdir, --suffix and --save_state may be given with other values")
+                   "only --max_steps, --outdir, --suffix, --save_state and --dist_backend may be given with other values")
+    p.add_argument("--dist_backend", type=str, default="nccl", choices=("nccl", "gloo"), help="under torchrun: the process group's backend; gloo lets "
+                   "several ranks share one GPU")
     return p
 
 
-RESUME_FREE = ("max_steps", "outdir", "suffix", "save_state", "resume")      # the flags a --resume may change
+RESUME_FREE = ("max_steps", "outdir", "suffix", "save_state", "resume", "dist_backend")      # the flags a --resume may change
 
 
 def check_supported(args):
@@ -147,9 +155,10 @@ def checkpoint_names(round_totals, every):
 
 
 def main(argv=None):
-    from . import run_state
+    from . import dist_run, run_state
     p = parser()
     args = p.parse_args(argv)
+    rank, world, local = dist_run.ranks()
     state = None
     if args.resume:
         state = run_state.load_state(p, args.resume, "pretrain")
@@ -157,6 +166,8 @@ def main(argv=None):
                                      "the solver, the incumbent and the search loop")
     if args.save_state and not args.outdir:
         p.error("--save_state 1 writes <outdir>/<suffix>/state.pt: it needs --outdir")
+    if world > 1 and not args.eval:                 # after a --resume: the saved run's population is the one that is split
+        dist_run.check_divisible(p, world, popsize=args.popsize)
     check_supported(args)
     if args.eval and not args.load:
         p.error("--eval 1 evaluates a gait: it needs --load X.npz")
@@ -165,13 +176,16 @@ def main(argv=None):
     if not args.eval and int(args.popsize * 0.1) < 1:
         p.error("--popsize %d: SimpleGA's elite_ratio 0.1 needs a population of at least 10 to keep one parent" % args.popsize)
     if args.eval:
-        return evaluate(args)
-    return pretrain(args) if state is None else pretrain(args, state)
+        return evaluate(args) if rank == 0 else []                     # --eval runs on rank 0 alone
+    if world == 1:
+        return pretrain(args) if state is None else pretrain(args, state)
+    with dist_run.process_group(world, local, getattr(args, "dist_backend", "nccl")) as dev:     # a state file may predate the flag
+        return pretrain(args, state, rank, world, dev)
 
 
-def make_eval_env(args, cfg):
+def make_eval_env(args, cfg, device=0):
     from .env import VecQuadrupedalEnv, apply_dynamic_param
-    return apply_dynamic_param(VecQuadrupedalEnv(args.eval_envs, auto_reset=False, **cfg), args.dynamic_param)
+    return apply_dynamic_param(VecQuadrupedalEnv(args.eval_envs, device=device, auto_reset=False, **cfg), args.dynamic_param)
 
 
 def evaluate(args):
@@ -188,9 +202,11 @@ def evaluate(args):
     return rec
 
 
-def pretrain(args, state=None):
-    """The search; `state`: a --save_state file to continue from (its solver, incumbent and counters replace the set-up)."""
+def pretrain(args, state=None, rank=0, world=1, dev=0):
+    """The search on this rank (device `dev`) of `world` ranks; returns the records rank 0 printed, [] on the other ranks.  `state`: a
+    --save_state file to continue from (its solver, incumbent and counters replace the set-up)."""
     import torch
+    import torch.distributed as dist
     from . import run_state
     from .env import apply_dynamic_param
     from .es import PopulationEvaluator, SimpleGA, solutions_to_etg_device
@@ -205,16 +221,20 @@ def pretrain(args, state=None):
     solver = SimpleGA(12, sigma_init=args.sigma, sigma_decay=args.sigma_decay, sigma_limit=0.005, elite_ratio=0.1, weight_decay=0.005,
                       popsize=args.popsize, param=init.copy())                                                  # pretrain.py:178-185
     cfg = env_config(args)
-    evaluator = PopulationEvaluator(args.popsize, args.es_rollouts, max_steps=ES_MAX_STEP + 1, policy=None, **cfg)
+    evaluator = PopulationEvaluator(args.popsize, args.es_rollouts, max_steps=ES_MAX_STEP + 1, rank=rank, world=world, device=dev, policy=None, **cfg)
     apply_dynamic_param(evaluator.env, args.dynamic_param)
-    eval_env = make_eval_env(args, cfg)
+    eval_env = make_eval_env(args, cfg, device=dev) if rank == 0 else None
     outdir = os.path.join(args.outdir, args.suffix)
-    os.makedirs(outdir, exist_ok=True)
+    if rank == 0:
+        os.makedirs(outdir, exist_ok=True)
     pop = args.popsize
 
     def rollout(ws, bs):
         fit, mlen, tmean, succ = evaluator.evaluate(ws, bs, terms=EVAL_TERMS)
-        steps = int(evaluator.len.sum())                          # the env steps these episodes took
+        steps = evaluator.len.sum()                               # the env steps these episodes took, over every rank's shard
+        if world > 1:
+            dist.all_reduce(steps)
+        steps = int(steps)
         return fit.double().cpu().numpy(), mlen.double().cpu().numpy(), tmean.double().cpu().numpy(), succ.double().cpu().numpy(), steps
 
     # the incumbent seeds best_param / best_reward (the train.py:395-396 rule; both are undefined in the reference).  This evaluation is set-up:
@@ -234,13 +254,15 @@ def pretrain(args, state=None):
     run_args = dict(vars(args))                          # what a --save_state file records
 
     def save_state():
+        if rank != 0:
+            return
         run_state.write_atomic(os.path.join(outdir, "state.pt"), {
             "command": "pretrain", "args": run_args, "solver": solver.state_dict(), "best_param": np.array(best_param), "best_reward": best_reward,
             "loop": {"test_flag": test_flag, "es_step": es_step, "env_steps": env_steps}})
     while env_steps < args.max_steps:
         for _ in range(args.es_train_steps):                                                                   # pretrain.py:221-256
             sol = solver.ask()
-            ws, bs = solutions_to_etg_device(sol, prior_points, w0, b0, ETG_T=args.ETG_T)
+            ws, bs = solutions_to_etg_device(sol, prior_points, w0, b0, ETG_T=args.ETG_T, device=dev)
             fit, mlen, tmean, succ, steps = rollout(ws.cpu().numpy(), bs.cpu().numpy())
             env_steps += steps
             fit = np.where(np.isfinite(fit), fit, -1e9)                  # a diverged rollout must lose, not poison tell()
@@ -256,9 +278,10 @@ def pretrain(args, state=None):
                 rec["episode_" + k], rec["mean_" + k] = ep, ep / mean_steps
             rec["success_rate"] = float(succ.mean())
             rec["env_steps"] = env_steps
-            log.append(rec); print(json.dumps(rec), flush=True)
+            if rank == 0:
+                log.append(rec); print(json.dumps(rec), flush=True)
         due, test_flag = eval_due(env_steps, test_flag, args.eval_every_steps)
-        if due:                                                                                                # pretrain.py:258-277
+        if due and rank == 0:                                                                                  # pretrain.py:258-277
             w, b, _ = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, w0=w0, b0=b0, points=prior_points + best_param.reshape(-1, 2))
             r = run_evaluate_episodes(eval_env, w, b, policy=None, max_step=EVAL_MAX_STEP)
             path = os.path.join(outdir, "itr_%d.npz" % env_steps)
@@ -270,7 +293,9 @@ def pretrain(args, state=None):
                 save_state()
     if args.save_state:
         save_state()
-    evaluator.env.close(); eval_env.close()
+    evaluator.env.close()
+    if eval_env is not None:
+        eval_env.close()
     return log
 
 

@@ -10,6 +10,14 @@ The reference's flags are honoured or refused before any device work (check_supp
     python -m paddlerobotics_b200.train --num_envs 4096 --max_steps 2000000 --ES 1
     python -m paddlerobotics_b200.train --train_eval_envs 16 --e_step_growth 50 --outdir train_log
     python -m paddlerobotics_b200.train --outdir ckpt --save_state 1; python -m paddlerobotics_b200.train --outdir ckpt --resume ckpt/exp0/state.pt --max_steps N
+    torchrun --nproc_per_node 8 -m paddlerobotics_b200.train --num_envs 32768 --batch 32768 --max_steps 16000000 --outdir ckpt
+
+Under torchrun (WORLD_SIZE > 1) --num_envs, --batch, --memory and --popsize stay global sizes, split evenly over the ranks: each rank steps
+its contiguous shard of the envs, keeps its own replay ring and samples its share of the batch; the data-parallel learner (sync "exact")
+all-reduces the gradients between its phases, so every rank holds the same weights.  The step counters and cadences stay global.  Rank r
+seeds torch with --seed + r (warm-up actions, exploration noise, --sensor_noise) and keys the learner's noise by r; NumPy's generator, which
+the ES solver draws from, gets --seed on every rank.  Only rank 0 prints, evaluates (--train_eval_envs, --eval) and writes checkpoints.
+--save_state / --resume run on one GPU only.
 """
 import argparse
 import json
@@ -19,8 +27,8 @@ import time
 import numpy as np
 import torch
 
-from . import _lib, run_state
-from .agent import MujocoAgent, SACLearner
+from . import _lib, dist_run, run_state
+from .agent import MujocoAgent, SACLearner, flatten_params
 from .env import VecQuadrupedalEnv, apply_dynamic_param
 from .es import PopulationEvaluator, SimpleGA, TrainEpisodeStats, solutions_to_etg_device
 from .etg import ETG_layer, Opt_with_points
@@ -83,6 +91,8 @@ def parser():
                    "--log_every, --outdir, --suffix and --save_state may be given with other values")
     p.add_argument("--e_step_growth", type=int, default=0, help="G > 0: every --eval_every_steps, `if e_step < 600: e_step += G` (train.py:384-385; the "
                    "reference's G is 50); 0 = a fixed --e_step")
+    p.add_argument("--dist_backend", type=str, default="nccl", choices=dist_run.BACKENDS, help="under torchrun: the process group's backend; gloo lets "
+                   "several ranks share one GPU, and needs --graph_iter 0 (a gloo collective cannot be captured in a CUDA graph)")
     # ---- the rest of the reference's flags (train.py:452-505), with its defaults
     p.add_argument("--act_mode", type=str, default="traj", choices=("traj", "pose", "torque"), help="motor mode and act_bound (train.py:279,315-320)")
     p.add_argument("--normal", type=int, default=1)
@@ -154,6 +164,17 @@ RESUME_FREE = ("max_steps", "log_every", "outdir", "suffix", "save_state", "resu
 RESUME_CONFLICTS = (("--load", "load"), ("--ETG_path", "ETG_path"), ("--eval 1", "eval"))
 
 
+def check_world(p, args, world):
+    """The refusals of a run over `world` > 1 ranks, raised before any device work."""
+    if args.save_state or args.resume:
+        raise NotImplementedError("--save_state / --resume with WORLD_SIZE %d: every rank's env shard, replay ring and generators would need their own "
+                                  "state file; run it on one GPU" % world)
+    dist_run.check_divisible(p, world, num_envs=args.num_envs, batch=args.batch, memory=args.memory, popsize=args.popsize)
+    if args.dist_backend == "gloo" and args.graph_iter:
+        p.error("--dist_backend gloo with --graph_iter 1: gloo collectives run on the host and cannot be captured in the iteration's CUDA graph; "
+                "give --graph_iter 0, or use nccl")
+
+
 def resume_args(p, argv, saved):
     """The arguments of a --resume run: the saved run's, with the RESUME_FREE flags of this command line.  Any other flag given on the
     command line with a value other than the saved one is an argument error (p.error) naming the flags, as are --load, --ETG_path and
@@ -215,38 +236,44 @@ def env_config(args):
                 etg_foot_y_inset=args.step_y if args.task_mode == "balancebeam" else 0.0, etg_T=float(args.ETG_T), etg_T2=float(args.ETG_T))
 
 
-def train_env_config(args):
+def train_env_config(args, rank=0):
     """env_config plus the observation, action and reward flags of this command (the make_env keywords of train.py:305-309).  Joint limits and
-    knee contacts stay off, as in every earlier version of this command (quadrupedal_config turns them on)."""
+    knee contacts stay off, as in every earlier version of this command (quadrupedal_config turns them on).  --sensor_noise draws from
+    --seed + rank."""
     from .env import SENSOR_NOISE_STDDEV, _motor_mode
     cfg = env_config(args)
     cfg.update(vel_d=float(args.vel_d), reward_p=float(args.reward_p), obs_normal=int(bool(args.normal)), action_filter=int(bool(args.enable_action_filter)),
                etg_enabled=int(bool(args.ETG)), motor_mode=_motor_mode(args.act_mode), sensor_dis=int(bool(args.sensor_dis)),
                sensor_contact=int(bool(args.sensor_contact)), sensor_imu=int(args.sensor_imu), sensor_motor=int(args.sensor_motor), sensor_etg=int(bool(args.sensor_ETG)))
     if args.sensor_noise:
-        cfg.update(noise_stdev=SENSOR_NOISE_STDDEV, noise_seed=int(args.seed))
+        cfg.update(noise_stdev=SENSOR_NOISE_STDDEV, noise_seed=int(args.seed) + rank)
     return cfg
 
 
-def make_envs(args, env_cfg, policy=None, act_bound=None):
-    """The training env and the ES phase's PopulationEvaluator (None without --ES), both on the --dynamic_param dynamics."""
-    env = apply_dynamic_param(VecQuadrupedalEnv(args.num_envs, auto_reset=True, max_episode_steps=args.e_step, **env_cfg), args.dynamic_param)
+def make_envs(args, env_cfg, policy=None, act_bound=None, rank=0, world=1, device=0):
+    """The training env (this rank's shard of --num_envs) and the ES phase's PopulationEvaluator (this rank's shard of the population; None
+    without --ES), both on the --dynamic_param dynamics."""
+    env = apply_dynamic_param(VecQuadrupedalEnv(args.num_envs // world, device=device, auto_reset=True, max_episode_steps=args.e_step, **env_cfg),
+                              args.dynamic_param)
     evaluator = None
     if args.ES:
-        evaluator = PopulationEvaluator(args.popsize, args.es_rollouts, max_steps=args.e_step, policy=policy,
+        evaluator = PopulationEvaluator(args.popsize, args.es_rollouts, max_steps=args.e_step, rank=rank, world=world, device=device, policy=policy,
                                         act_bound=args.act_bound if act_bound is None else act_bound, **env_cfg)
         apply_dynamic_param(evaluator.env, args.dynamic_param)
     return env, evaluator
 
 
-def make_eval_env(args, env_cfg, n):
+def make_eval_env(args, env_cfg, n, device=0):
     """An env of n envs without auto-reset on the training configuration and the --dynamic_param dynamics (--eval, --train_eval_envs)."""
-    return apply_dynamic_param(VecQuadrupedalEnv(n, auto_reset=False, **env_cfg), args.dynamic_param)
+    return apply_dynamic_param(VecQuadrupedalEnv(n, device=device, auto_reset=False, **env_cfg), args.dynamic_param)
 
 
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    rank, world, local = dist_run.ranks()
+    if world > 1:
+        check_world(p, args, world)
     state = None
     if args.resume:
         state = run_state.load_state(p, args.resume, "train")
@@ -254,12 +281,8 @@ def main(argv=None):
     if args.save_state and not args.outdir:
         p.error("--save_state 1 writes <outdir>/<suffix>/state.pt: it needs --outdir")
     check_supported(args)
-    torch.manual_seed(args.seed); np.random.seed(args.seed)
-    n = args.num_envs
-    layer = ETG_layer(args.ETG_T, 0.026, 20, 0.04, np.array([-np.pi / 2, 0]), 0.2, args.ETG_T)
-    w0, b0, prior_points = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, Footheight=args.footheight, Steplength=args.steplen)     # train.py:298-299
-    w, b = w0, b0
-    env_cfg = train_env_config(args)
+    torch.manual_seed(args.seed + rank); np.random.seed(args.seed)
+    env_cfg = train_env_config(args, rank)
     run_args = dict(vars(args))                      # what a --save_state file records
     if state is not None:
         args = argparse.Namespace(**run_args)
@@ -269,30 +292,70 @@ def main(argv=None):
     if args.eval and not args.load:
         p.error("--eval 1 evaluates a checkpoint: it needs --load itr_*.pt")
     check_args(p, args)
-    from .bctrain import act_bound_of
-    bound = act_bound_of(args)                                                                                                    # train.py:315-320
-    # a uniform bound stays a Python scalar: the same float32 products as before the per-motor bounds of --act_mode pose
-    bound = float(bound[0]) if np.all(bound == bound[0]) else torch.as_tensor(bound, dtype=torch.float32, device="cuda")
     if args.eval:
-        return evaluate(args, env_cfg, bound)
+        if rank != 0:
+            return []                                                                                                             # --eval runs on rank 0 alone
+        world = 1
+    with dist_run.process_group(world, local, getattr(args, "dist_backend", "nccl")) as dev:     # a state file may predate the flag
+        from .bctrain import act_bound_of
+        bound = act_bound_of(args)                                                                                                # train.py:315-320
+        # a uniform bound stays a Python scalar: the same float32 products as before the per-motor bounds of --act_mode pose
+        bound = float(bound[0]) if np.all(bound == bound[0]) else torch.as_tensor(bound, dtype=torch.float32, device=torch.device("cuda", dev))
+        if args.eval:
+            return evaluate(args, env_cfg, bound)
+        return run(args, env_cfg, bound, state, run_args, rank, world, dev)
+
+
+def run(args, env_cfg, bound, state, run_args, rank=0, world=1, dev=0):
+    """The training loop on this rank (device `dev`) of `world` ranks; returns the records rank 0 printed, [] on the other ranks.  `state`: a
+    --save_state file to continue from (one rank only)."""
+    import torch.distributed as dist
+    layer = ETG_layer(args.ETG_T, 0.026, 20, 0.04, np.array([-np.pi / 2, 0]), 0.2, args.ETG_T)
+    w0, b0, prior_points = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, Footheight=args.footheight, Steplength=args.steplen)     # train.py:298-299
+    n_all = args.num_envs                       # the global env count: what `total` advances by per iteration
+    n = n_all // world                          # this rank's shard
+    key = rank << 40                            # the rank's offset of every counter-RNG seed: rank 0 keeps the single-GPU keys
+
+    def say(rec, keep=True):
+        if rank == 0:
+            if keep:
+                log.append(rec)
+            print(json.dumps(rec), flush=True)
+
+    def all_sum(t):
+        if world > 1:
+            dist.all_reduce(t)
+        return t
+
+    def warm():
+        # train.py:141's rpm.size() >= WARMUP_STEPS over the global ring: until the first learn every rank has appended the same rows, and
+        # afterwards the ring only grows, so W x this rank's fill level decides it on every rank alike without a collective
+        return rpm.size() * world >= args.warmup_steps
+
+    def check_replicas():
+        if world > 1 and not dist_run.all_equal(learner.replica_state()):
+            raise RuntimeError("the ranks' learners differ: the data-parallel update must leave every rank with the same weights and moments")
     # the evaluator's policy reads `learner` when it runs, so it may be built before the learner
-    env, evaluator = make_envs(args, env_cfg, policy=lambda o: learner.actor.forward(o)[0][0], act_bound=bound)
-    eval_env = make_eval_env(args, env_cfg, args.train_eval_envs) if args.train_eval_envs else None
+    env, evaluator = make_envs(args, env_cfg, policy=lambda o: learner.actor.forward(o)[0][0], act_bound=bound, rank=rank, world=world, device=dev)
+    eval_env = make_eval_env(args, env_cfg, args.train_eval_envs, device=dev) if args.train_eval_envs and rank == 0 else None
     od = env.observation_dim
-    agent = MujocoAgent(od, 12, seed=args.seed)
+    agent = MujocoAgent(od, 12, device=dev, seed=args.seed)
     ETG_best_param, w, b = initial_etg(args)                                                                                      # ES_solver.get_best_param(), train.py:348
     if args.load:
         agent.restore(args.load)
         z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
         w, b, ETG_best_param = z["w"], z["b"], z["param"].reshape(-1)
-    outdir = os.path.join(args.outdir, args.suffix) if args.outdir else ""
+    outdir = os.path.join(args.outdir, args.suffix) if args.outdir and rank == 0 else ""
     if outdir:
         os.makedirs(outdir, exist_ok=True)
-    ckpt_every = args.eval_every_steps or int(1e4) * n
+    ckpt_every = args.eval_every_steps or int(1e4) * n_all
     test_flag = 1
     e_step = args.e_step
-    learner = SACLearner(agent, args.batch, gamma=GAMMA, tau=TAU, alpha=ALPHA, actor_lr=ACTOR_LR, critic_lr=CRITIC_LR)
-    rpm = ReplayMemory(args.memory, od, 12, device_cursor=bool(args.graph_iter and args.overlap))
+    batch = args.batch // world
+    learner = SACLearner(agent, batch, gamma=GAMMA, tau=TAU, alpha=ALPHA, actor_lr=ACTOR_LR, critic_lr=CRITIC_LR, world=world, seed_key=key)
+    if world > 1 and not dist_run.all_equal(torch.cat(flatten_params(agent.params))):
+        raise RuntimeError("the ranks built different agents from --seed %d" % args.seed)
+    rpm = ReplayMemory(args.memory // world, od, 12, device=dev, device_cursor=bool(args.graph_iter and args.overlap))
     solver = SimpleGA(12, sigma_init=args.sigma, sigma_decay=args.sigma_decay, sigma_limit=0.005, elite_ratio=0.1, weight_decay=0.005,
                       popsize=args.popsize, param=ETG_best_param.copy())                                                          # train.py:288-295
     obs = env.reset(w, b).clone()
@@ -316,7 +379,6 @@ def main(argv=None):
         L = state["loop"]
         total, it, last_es, test_flag, e_step, last_log = L["total"], L["it"], L["last_es"], L["test_flag"], L["e_step"], (L["last_log_total"], 0.0)
         ETG_best_param, w, b = state["ETG_best_param"], state["w"], state["b"]
-        losses = learner.losses
         torch.set_rng_state(state["torch_rng"]); torch.cuda.set_rng_state(state["cuda_rng"], env.device)
 
     def save_state():
@@ -330,7 +392,7 @@ def main(argv=None):
     def graph_iteration():
         cur = torch.cuda.current_stream()
         act = learner.actor.forward(obs, mode=1, eps=torch.randn(n, 12, device=env.device))[0][0]     # agent.sample(obs)
-        batch_t = rpm.sample_batch(args.batch, out=learner.static_batch())
+        batch_t = rpm.sample_batch(batch, out=learner.static_batch())
         s_learn.wait_stream(cur)
         with torch.cuda.stream(s_learn):
             learner.learn(*batch_t, graph=False, pull=False)
@@ -361,33 +423,33 @@ def main(argv=None):
         if iter_graph is not None:
             iter_graph.replay()
             rpm.advance(n)
-            rew, done, losses = env.reward, env.done, learner.losses
-            total += n; it += 1
+            rew, done = env.reward, env.done
+            total += n_all; it += 1
         else:
-            if rpm.size() < args.warmup_steps:
+            if not warm():
                 act = torch.rand(n, 12, device=env.device) * 2 - 1                         # train.py:141-142
             else:
-                act = learner.actor.forward(obs, mode=1, seed=it + 1)[0][0]               # agent.sample(obs)
-            learning = rpm.size() >= args.warmup_steps
+                act = learner.actor.forward(obs, mode=1, seed=it + 1 + key)[0][0]         # agent.sample(obs)
+            learning = warm()
             if learning and args.overlap:
                 # the learner step (latency-bound small kernels) runs on its own stream NEXT TO the env step (one warp per scheduler):
                 # it samples transitions up to t-1 and its new weights are first used by the policy forward of step t+1, exactly as
                 # in the sequential order, except that transition t itself joins the replay one update later
-                batch_t = rpm.sample_batch(args.batch, out=learner.static_batch())
+                batch_t = rpm.sample_batch(batch, out=learner.static_batch())
                 s_learn.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(s_learn):
                     for x in batch_t:
                         x.record_stream(s_learn)
-                    losses = learner.learn(*batch_t, graph=True, pull=False)
+                    learner.learn(*batch_t, graph=True, pull=False)
             nobs, rew, done, info = env.step(act * bound)
             stats.step(rew, done, info, env._stream())
             rpm.append(obs, act, rew, nobs, 1.0 - done.float())                            # terminal = 1 - done, train.py:148-149,159
             if learning and args.overlap:
                 torch.cuda.current_stream().wait_stream(s_learn)
             obs.copy_(nobs)
-            total += n; it += 1
-            if rpm.size() >= args.warmup_steps and not (learning and args.overlap):
-                losses = learner.learn(*rpm.sample_batch(args.batch, out=learner.static_batch()), graph=True, pull=False)   # one update per control step, train.py:163-169
+            total += n_all; it += 1
+            if warm() and not (learning and args.overlap):
+                learner.learn(*rpm.sample_batch(batch, out=learner.static_batch()), graph=True, pull=False)   # one update per control step, train.py:163-169
             if args.graph_iter and args.overlap and learning and it % args.log_every != 0:
                 # warm-up is over and one eager learning iteration has run: capture the iteration once
                 iter_graph = capture_iteration()
@@ -395,23 +457,28 @@ def main(argv=None):
             torch.cuda.synchronize()
             el = time.perf_counter() - t0
             rate_int = (total - last_log[0]) / max(el - last_log[1], 1e-9); last_log = (total, el)
-            ep = stats.take()
+            ep = stats.take() if world == 1 else stats.take(all_sum)
+            if world == 1:
+                step_rew, done_frac, loss = float(rew.mean()), float(done.float().mean()), learner.losses
+            else:                                   # global means: the envs of every rank, the shard losses averaged
+                g = all_sum(torch.cat([torch.stack([rew.double().sum(), done.double().sum()]), learner.losses[:2].double()])).tolist()
+                step_rew, done_frac, loss = g[0] / n_all, g[1] / n_all, (g[2] / world, g[3] / world)
             closed = ep["episodes"] + ep["nonfinite_episodes"] > 0
-            rec = {"env_steps": total, "iters": it, "env_steps_per_s": total / el, "interval_env_steps_per_s": rate_int, "mean_step_reward": float(rew.mean()), "done_frac": float(done.float().mean()),
+            rec = {"env_steps": total, "iters": it, "env_steps_per_s": total / el, "interval_env_steps_per_s": rate_int, "mean_step_reward": step_rew, "done_frac": done_frac,
                    "episode_return": ep["return"],
-                   "critic_loss": float(losses[0]) if rpm.size() >= args.warmup_steps else None, "actor_loss": float(losses[1]) if rpm.size() >= args.warmup_steps else None,
+                   "critic_loss": float(loss[0]) if warm() else None, "actor_loss": float(loss[1]) if warm() else None,
                    "train_episodes": ep["episodes"] if closed else None, "train_nonfinite_episodes": ep["nonfinite_episodes"] if closed else None,
                    "train_episode_step": ep["length"]}
             for k in EVAL_TERMS:
                 rec["train_episode_" + k], rec["train_mean_" + k] = ep["terms"][k], ep["mean_terms"][k]
             rec["train_success_rate"] = ep["success_rate"]
-            log.append(rec); print(json.dumps(rec), flush=True)
+            say(rec)
         due, test_flag = block_due(total, test_flag, ckpt_every)
         if due:                                                                         # train.py:370-390, in its order
             if eval_env is not None:
                 r = run_evaluate_episodes(eval_env, w, b, policy=lambda o: learner.actor.forward(o)[0][0], act_bound=bound, max_step=EVAL_MAX_STEP)
-                rec = eval_record(total, r, e_step)
-                log.append(rec); print(json.dumps(rec), flush=True)
+                say(eval_record(total, r, e_step))
+            check_replicas()     # its all-gather is also where the other ranks wait for rank 0's evaluation
             if args.e_step_growth:
                 grown = grow_e_step(e_step, args.e_step_growth)
                 if grown != e_step:
@@ -422,20 +489,20 @@ def main(argv=None):
                 learner.pull()
                 agent.save(os.path.join(outdir, "itr_%d.pt" % total))
                 np.savez(os.path.join(outdir, "itr_%d.npz" % total), w=w, b=b, param=ETG_best_param)
-        if evaluator is not None and total - last_es >= args.es_every_steps and rpm.size() >= args.warmup_steps:
+        if evaluator is not None and total - last_es >= args.es_every_steps and warm():
             last_es = total
             # the incumbent ETG seeds best_reward (train.py:395-396): a sampled individual replaces it only if it is actually better
             es_replay = rpm if args.es_rpm else None
             # popsize copies of ONE gait: only one episode goes to the replay (train.py:395)
             inc_fit, _ = evaluator.evaluate(np.repeat(np.asarray(w)[None], args.popsize, 0), np.repeat(np.asarray(b)[None], args.popsize, 0),
                                             replay=es_replay, record=np.arange(args.popsize) == 0)
-            es_rows = [int(evaluator.rows)] if args.es_rpm else []
+            es_rows = [int(all_sum(evaluator.rows.clone()))] if args.es_rpm else []
             inc = inc_fit.double().cpu().numpy()
             best_fit = float(np.nanmean(inc)) if np.isfinite(inc).any() else -np.inf
             best_param = ETG_best_param.copy()
             for gen in range(args.es_train_steps):                                     # train.py:397-418
                 sol = solver.ask()
-                ws, bs = solutions_to_etg_device(sol, prior_points, w0, b0, ETG_T=args.ETG_T)
+                ws, bs = solutions_to_etg_device(sol, prior_points, w0, b0, ETG_T=args.ETG_T, device=dev)
                 fit, mlen = evaluator.evaluate(ws.cpu().numpy(), bs.cpu().numpy(), replay=es_replay)
                 fit_np = fit.double().cpu().numpy()
                 fit_np = np.where(np.isfinite(fit_np), fit_np, -1e9)                    # a diverged rollout must lose, not poison tell()
@@ -444,13 +511,14 @@ def main(argv=None):
                     best_fit, best_param = float(fit_np.max()), np.asarray(sol[int(fit_np.argmax())]).copy()
                 rec = {"ES_gen": gen, "fitness_max": float(fit_np.max()), "fitness_mean": float(fit_np.mean()), "mean_len": float(mlen.mean())}
                 if args.es_rpm:
-                    es_rows.append(int(evaluator.rows))
+                    es_rows.append(int(all_sum(evaluator.rows.clone())))
                     rec["rpm_rows"] = es_rows[-1]
-                print(json.dumps(rec), flush=True)
+                say(rec, keep=False)
             if args.es_rpm:
                 # the masked appends advanced the ring's device cursor; one read brings the host mirrors level before the loop uses them
                 rpm.sync_host()
-                print(json.dumps({"ES_rpm_rows": sum(es_rows), "env_steps": total, "rpm_size": rpm.size()}), flush=True)
+                rpm_size = rpm.size() if world == 1 else int(all_sum(torch.tensor(rpm.size(), device=env.device)))
+                say({"ES_rpm_rows": sum(es_rows), "env_steps": total, "rpm_size": rpm_size}, keep=False)
             ETG_best_param = best_param
             pts = prior_points + ETG_best_param.reshape(-1, 2)                          # train.py:433-437
             w, b, _ = Opt_with_points(ETG=layer, ETG_T=args.ETG_T, w0=w0, b0=b0, points=pts)
@@ -462,6 +530,7 @@ def main(argv=None):
         save_state()
     torch.cuda.synchronize()
     learner.pull()
+    check_replicas()
     if eval_env is not None:
         eval_env.close()
     return log
