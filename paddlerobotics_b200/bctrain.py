@@ -25,7 +25,7 @@ import torch
 from . import bc
 from .agent import MujocoAgent, SACLearner
 from .env import VecQuadrupedalEnv, apply_dynamic_param, etg_of_path, quadrupedal_config
-from .train import EVAL_TERMS
+from .train import frame_writer, run_evaluate_episodes
 
 ACTOR_LR, CRITIC_LR = 3e-4, 3e-4            # BCtrain.py:44-45
 EVAL_STEPS, RANDOM_EVAL_STEPS = 600, 800    # run_evaluate_episodes(agent, env, 600, ...) BCtrain.py:321; run_random_eval(..., 800, ...) :302
@@ -162,35 +162,6 @@ def make_vec_env(args, n, auto_reset, max_episode_steps=0):
     return apply_dynamic_param(env, args.dynamic_param)
 
 
-def run_episodes(env, policy, w, b, act_bound, max_step, x_noise=0, render=None):
-    """One episode per env (no auto-reset), at most max_step + 1 control steps (donef = steps > max_step, BCtrain.py:161).  Return,
-    length and the per-term sums freeze at each env's first done (b2q_es_accumulate, as train.evaluate).  render(steps): per-step hook."""
-    from . import _lib
-    from ._config import INFO
-    lib, dev, n, es, stream = _lib.load(), env.device, env.num_envs, env.obs.element_size(), env._stream()
-    nt = len(EVAL_TERMS)
-    cols = torch.tensor([INFO[k] for k in EVAL_TERMS], device=dev)
-    alive = torch.ones(n, dtype=torch.uint8, device=dev)
-    ret, length = torch.zeros(n, dtype=env.dtype, device=dev), torch.zeros(n, dtype=torch.int32, device=dev)
-    t_alive, t_sum, t_len = torch.empty(nt, n, dtype=torch.uint8, device=dev), torch.zeros(nt, n, dtype=env.dtype, device=dev), torch.zeros(nt, n, dtype=torch.int32, device=dev)
-    t_val = torch.empty(nt, n, dtype=env.dtype, device=dev)
-    xo = np.random.uniform(-0.1, 0.1, n) if x_noise else None
-    obs = env.reset(w, b, x_offset=xo)
-    for steps in range(1, max_step + 2):
-        obs, rew, done, info = env.step(policy(obs, steps) * act_bound, donef=steps > max_step)
-        if render is not None:
-            render(steps)
-        t_val.copy_(info.index_select(1, cols).T)
-        t_alive.copy_(alive.expand(nt, n))
-        for j in range(nt):
-            assert lib.b2q_es_accumulate(t_val[j].data_ptr(), done.data_ptr(), t_alive[j].data_ptr(), t_sum[j].data_ptr(), t_len[j].data_ptr(), n, es, stream) == 0
-        assert lib.b2q_es_accumulate(rew.data_ptr(), done.data_ptr(), alive.data_ptr(), ret.data_ptr(), length.data_ptr(), n, es, stream) == 0
-        if not bool(alive.any()):
-            break
-    return {"mean_return": float(ret.double().mean()), "mean_length": float(length.double().mean()),
-            "terms": {k: float(t_sum[j].double().mean()) for j, k in enumerate(EVAL_TERMS)}}
-
-
 def main(argv=None):
     from . import run_state
     p = parser()
@@ -305,10 +276,12 @@ def random_eval(args, learner, expert, env, w, b, bound):
     800 steps each; ref_ratio = student return / expert return."""
     noise = bool(args.sensor_noise)
     obs_mem = bc.BCReplayMemory(1, 46, 49, device=env.device)       # observe(append=False) never touches its ring
-    # noise keys of the evaluation steps: step words from 2^30 up, apart from the training steps' 0, 1, 2, ...
-    stu = run_episodes(env, lambda o, s: learner.actor.forward(obs_mem.observe(o, 1 << 30 | s, noise=noise, append=False, seed=args.seed), mode=0)[0][0],
-                       w, b, bound, RANDOM_EVAL_STEPS)
-    ref = run_episodes(env, lambda o, s: expert.predict_batch(o), w, b, bound, RANDOM_EVAL_STEPS)
+
+    def student(o, s):
+        # noise keys of the evaluation steps: step words from 2^30 up, apart from the training steps' 0, 1, 2, ...
+        return learner.actor.forward(obs_mem.observe(o, 1 << 30 | s, noise=noise, append=False, seed=args.seed), mode=0)[0][0]
+    stu = run_evaluate_episodes(env, w, b, policy=student, act_bound=bound, max_step=RANDOM_EVAL_STEPS)
+    ref = run_evaluate_episodes(env, w, b, policy=lambda o, s: expert.predict_batch(o), act_bound=bound, max_step=RANDOM_EVAL_STEPS)
     return {"eval_return": stu["mean_return"], "eval_length": stu["mean_length"], "ref_return": ref["mean_return"], "ref_length": ref["mean_length"],
             "ref_ratio": stu["mean_return"] / ref["mean_return"] if ref["mean_return"] != 0 else None, "terms": stu["terms"]}
 
@@ -316,18 +289,12 @@ def random_eval(args, learner, expert, env, w, b, bound):
 def evaluate(args, student, w, b, bound):
     """--eval 1 --load X.pt: run_evaluate_episodes (BCtrain.py:147-176,317-326) — the student's deterministic episode, at most 600 steps, on
     its (noisy) obs[3:]; one JSON line; --render_dir writes img{step}.png of env 0."""
-    from .render import write_png
     env = make_vec_env(args, args.eval_envs, auto_reset=False)
     obs_mem = bc.BCReplayMemory(1, 46, 49, device=env.device)
-    if args.render_dir:
-        os.makedirs(args.render_dir, exist_ok=True)
-
-    def frame(steps):
-        rgba = env.get_camera_image(args.render_width, args.render_height, env_ids=[0])[0]
-        write_png(os.path.join(args.render_dir, "img%d.png" % steps), rgba[0].cpu().numpy())
-    rec = run_episodes(env, lambda o, s: student.predict_batch(obs_mem.observe(o, s, noise=bool(args.sensor_noise), append=False, seed=args.seed)),
-                       w, b, bound, EVAL_STEPS, x_noise=args.x_noise, render=frame if args.render_dir else None)
-    rec = {"eval_envs": args.eval_envs, **rec}
+    xo = np.random.uniform(-0.1, 0.1, args.eval_envs) if args.x_noise else None
+    r = run_evaluate_episodes(env, w, b, policy=lambda o, s: student.predict_batch(obs_mem.observe(o, s, noise=bool(args.sensor_noise), append=False, seed=args.seed)),
+                              act_bound=bound, max_step=EVAL_STEPS, x_offset=xo, render=frame_writer(env, args) if args.render_dir else None)
+    rec = {"eval_envs": args.eval_envs, "mean_return": r["mean_return"], "mean_length": r["mean_length"], "terms": r["terms"]}
     print(json.dumps(rec), flush=True)
     env.close()
     return rec

@@ -476,7 +476,7 @@ def run(args, env_cfg, bound, state, run_args, rank=0, world=1, dev=0):
         due, test_flag = block_due(total, test_flag, ckpt_every)
         if due:                                                                         # train.py:370-390, in its order
             if eval_env is not None:
-                r = run_evaluate_episodes(eval_env, w, b, policy=lambda o: learner.actor.forward(o)[0][0], act_bound=bound, max_step=EVAL_MAX_STEP)
+                r = run_evaluate_episodes(eval_env, w, b, policy=lambda o, s: learner.actor.forward(o)[0][0], act_bound=bound, max_step=EVAL_MAX_STEP)
                 say(eval_record(total, r, e_step))
             check_replicas()     # its all-gather is also where the other ranks wait for rank 0's evaluation
             if args.e_step_growth:
@@ -551,11 +551,13 @@ EVAL_MAX_STEP = 600                                                         # ru
 EVAL_TERMS = ("torso", "feet", "up", "tau", "badfoot", "footcontact")       # the info terms summed per episode, train.py:202-207
 
 
-def run_evaluate_episodes(env, w, b, policy=None, act_bound=0.3, max_step=EVAL_MAX_STEP, render=None):
-    """run_evaluate_episodes (train.py:182-211): one episode per env of `env` (no auto-reset) on the ETG (w, b), at most max_step + 1
-    control steps (the reference's loop breaks after step max_step + 1; donef forces the done flag of that step).  policy(obs) -> [N,12]
-    in [-1, 1], scaled by act_bound; None = zero residual (the open-loop ETG).  Each env's return, length, EVAL_TERMS sums and velx
-    success count freeze at its first done, all in one b2q_es_accumulate_terms launch per step.  render(steps): per-step hook.
+def run_evaluate_episodes(env, w, b, policy=None, act_bound=0.3, max_step=EVAL_MAX_STEP, x_offset=None, render=None):
+    """run_evaluate_episodes (train.py:182-211, BCtrain.py:147-176): one episode per env of `env` (no auto-reset) on the ETG (w, b), at most
+    max_step + 1 control steps (the reference's loop breaks after step max_step + 1; donef forces the done flag of that step).
+    policy(obs, steps) -> [N,12] in [-1, 1], scaled by act_bound, with steps the 1-based control step (bctrain keys the student's sensor
+    noise by it); None = zero residual (the open-loop ETG).  x_offset: [N] start displacements along x for env.reset (bctrain --x_noise 1).
+    Each env's return, length, EVAL_TERMS sums and velx success count freeze at its first done, all in one b2q_es_accumulate_terms launch
+    per step.  render(steps): per-step hook.
     Returns {mean_return, mean_length, terms: {term: mean episode sum}, success_rate: mean over envs of count / length}."""
     from . import _lib
     from .es import EpisodeStats
@@ -563,9 +565,9 @@ def run_evaluate_episodes(env, w, b, policy=None, act_bound=0.3, max_step=EVAL_M
     stats = EpisodeStats(_lib.load(), n, env.dtype, env.device, EVAL_TERMS)
     stream = env._stream()
     zero = torch.zeros(n, 12, dtype=env.dtype, device=env.device) if policy is None else None
-    obs = env.reset(w, b)
+    obs = env.reset(w, b, x_offset=x_offset)
     for steps in range(1, max_step + 2):
-        act = zero if policy is None else policy(obs) * act_bound                                        # agent.predict(obs), train.py:193
+        act = zero if policy is None else policy(obs, steps) * act_bound                                 # agent.predict(obs), train.py:193
         obs, rew, done, info = env.step(act, donef=steps > max_step)
         if render is not None:
             render(steps)
@@ -597,7 +599,7 @@ def evaluate(args, env_cfg, act_bound):
     agent.restore(args.load)
     z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
     w, b = z["w"], z["b"]
-    r = run_evaluate_episodes(env, w, b, policy=agent.predict_batch, act_bound=act_bound, max_step=EVAL_MAX_STEP,
+    r = run_evaluate_episodes(env, w, b, policy=lambda o, s: agent.predict_batch(o), act_bound=act_bound, max_step=EVAL_MAX_STEP,
                               render=frame_writer(env, args) if args.render_dir else None)
     rec = {"eval_envs": n, "mean_return": r["mean_return"], "mean_length": r["mean_length"], "terms": r["terms"]}
     print(json.dumps(rec), flush=True)

@@ -72,7 +72,7 @@ def eval_block(k):
     out = []
     for _ in range(3):
         torch.cuda.synchronize(); t0 = time.perf_counter()
-        r = train.run_evaluate_episodes(env, w, b, policy=agent.predict_batch, act_bound=0.3, max_step=train.EVAL_MAX_STEP)
+        r = train.run_evaluate_episodes(env, w, b, policy=lambda o, s: agent.predict_batch(o), act_bound=0.3, max_step=train.EVAL_MAX_STEP)
         torch.cuda.synchronize(); out.append((time.perf_counter() - t0, r["mean_length"]))
     env.close()
     return out
