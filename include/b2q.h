@@ -150,6 +150,15 @@ int64_t b2q_launch_count(B2QHandle h);
  * value of b2q_create. */
 int b2q_set_max_episode_steps(B2QHandle h, int max_episode_steps);
 
+/* Terrain atlas: env i of a height-field handle (terrain_type 1) reads tile tile_of_env[i] of `n_tiles` height fields instead of the
+ * create-time one.  Every tile lies on the handle's grid (hf_nx, hf_ny, hf_x0, hf_y0, hf_cell).  tiles_host is a HOST array
+ * [n_tiles][hf_ny][hf_nx], tile_of_env a HOST array [N] of indices in [0, n_tiles); both are copied.  The call waits for the stream,
+ * replaces any earlier atlas, and re-settles every env's reset snapshot on its tile with the dynamics it has: call b2q_reset before the
+ * next step.  From then on the handle runs the atlas kernels, in which env i computes what a plain height-field handle created on tile
+ * tile_of_env[i] computes.  Returns B2Q_EINVAL for a plane handle, n_tiles < 1 or an index out of range.  An atlas handle refuses
+ * b2q_snapshot_save, b2q_snapshot_load and b2q_render with B2Q_EINVAL. */
+int b2q_set_terrain_tiles(B2QHandle h, const double* tiles_host, int n_tiles, const int32_t* tile_of_env, void* stream);
+
 /* Whole-handle snapshot, for stopping a run and continuing it bit for bit.  The blob holds everything a later b2q_step / b2q_reset
  * reads: the SoA pool (state, snapshot, snap_obs, param, ETG packs, observation ring, position history, external force, step
  * counters) and the handle's mutable host fields (max_episode_steps).  It starts with a header: magic, format version, sizes,

@@ -36,6 +36,7 @@ SYMBOLS = {
     "b2q_snapshot_bytes": (C.c_int64, [_vp]),
     "b2q_snapshot_save": (_i, [_vp, _vp, _vp]),
     "b2q_snapshot_load": (_i, [_vp, _vp, _vp]),
+    "b2q_set_terrain_tiles": (_i, [_vp, _vp, _i, _vp, _vp]),
     # policy / critic MLP forward on wgmma tensor cores — include/b2q_mlp.h
     "b2q_mlp_create": (_i, [_i, _i, _i, _i, C.POINTER(_vp)]),
     "b2q_mlp_destroy": (_i, [_vp]),

@@ -89,9 +89,24 @@ __device__ __forceinline__ void emit_obs_block(const Model<T>& md, const T* stag
   for (int i = threadIdx.x; i < rows * od; i += blockDim.x) { int r = i / od, j = i - r * od; dst[i] = obs_out_elem(md, stage + r * OBS_DIM, j); }
 }
 
-template <typename T, int FEAT>
-__global__ void __launch_bounds__(128) b2q_step_kernel(Cfg<T> cf, const Model<T>* __restrict__ gm, Buffers<T> B, const T* __restrict__ action, int donef,
-                                                       int auto_reset, T* __restrict__ obs, T* __restrict__ reward, uint8_t* __restrict__ done, T* __restrict__ info) {
+// Terrain atlas (b2q_set_terrain_tiles): T height-field tiles on the handle's one hf_* grid, and the tile each env reads.  The TILES = 1
+// bodies below load env i's tile once per launch and step or settle it on a Cfg whose `hf` is that tile's base pointer (a 64-bit offset),
+// so terrain_height runs unchanged and env i computes what a plain height-field handle built on tile tile_of_env[i] computes.  They are
+// kernels of their own (b2q_step_tiles_kernel, b2q_settle_tiles_kernel): the default kernels' code does not change.
+struct Tiles {
+  const int32_t* tile_of_env;   // [N]
+  long long tile_elems;         // hf_nx * hf_ny
+};
+template <typename T, int TILES>
+__device__ __forceinline__ Cfg<T> env_cfg(const Cfg<T>& cf, const Tiles& tl, int env) {
+  Cfg<T> c = cf;
+  if constexpr (TILES != 0) c.hf = cf.hf + (size_t)tl.tile_of_env[env] * (size_t)tl.tile_elems;
+  return c;
+}
+
+template <typename T, int FEAT, int TILES>
+__device__ __forceinline__ void step_cta(const Cfg<T>& cf, const Tiles& tl, const Model<T>* __restrict__ gm, const Buffers<T>& B, const T* __restrict__ action,
+                                         int donef, int auto_reset, T* __restrict__ obs, T* __restrict__ reward, uint8_t* __restrict__ done, T* __restrict__ info) {
 #ifdef B2Q_REGION_CLOCKS
   const long long t_entry = clock64();
 #endif
@@ -117,7 +132,12 @@ __global__ void __launch_bounds__(128) b2q_step_kernel(Cfg<T> cf, const Model<T>
 #ifdef B2Q_REGION_CLOCKS
   cm.t_mark = t_entry;
 #endif
-  step_lane<T, FEAT>(cm, cf, md, B, env, valid, action, donef, auto_reset, stage + (ptrdiff_t)(srow - env) * OBS_DIM, reward, done, istage, env0, env0);
+  if constexpr (TILES != 0) {
+    step_lane<T, FEAT>(cm, env_cfg<T, TILES>(cf, tl, env), md, B, env, valid, action, donef, auto_reset, stage + (ptrdiff_t)(srow - env) * OBS_DIM, reward, done, istage,
+                       env0, env0);
+  } else {
+    step_lane<T, FEAT>(cm, cf, md, B, env, valid, action, donef, auto_reset, stage + (ptrdiff_t)(srow - env) * OBS_DIM, reward, done, istage, env0, env0);
+  }
   __syncthreads();
   const int rows = min(per_cta, B.N - env0);
   emit_obs_block(md, stage, obs, env0, rows);
@@ -135,7 +155,19 @@ __global__ void __launch_bounds__(128) b2q_step_kernel(Cfg<T> cf, const Model<T>
 }
 
 template <typename T, int FEAT>
-__global__ void __launch_bounds__(128) b2q_settle_kernel(Cfg<T> cf, const Model<T>* __restrict__ gm, Buffers<T> B, const uint8_t* __restrict__ mask) {
+__global__ void __launch_bounds__(128) b2q_step_kernel(Cfg<T> cf, const Model<T>* __restrict__ gm, Buffers<T> B, const T* __restrict__ action, int donef,
+                                                       int auto_reset, T* __restrict__ obs, T* __restrict__ reward, uint8_t* __restrict__ done, T* __restrict__ info) {
+  step_cta<T, FEAT, 0>(cf, Tiles{nullptr, 0}, gm, B, action, donef, auto_reset, obs, reward, done, info);
+}
+template <typename T, int FEAT>
+__global__ void __launch_bounds__(128) b2q_step_tiles_kernel(Cfg<T> cf, Tiles tl, const Model<T>* __restrict__ gm, Buffers<T> B, const T* __restrict__ action,
+                                                             int donef, int auto_reset, T* __restrict__ obs, T* __restrict__ reward, uint8_t* __restrict__ done,
+                                                             T* __restrict__ info) {
+  step_cta<T, FEAT, 1>(cf, tl, gm, B, action, donef, auto_reset, obs, reward, done, info);
+}
+
+template <typename T, int FEAT, int TILES>
+__device__ __forceinline__ void settle_cta(const Cfg<T>& cf, const Tiles& tl, const Model<T>* __restrict__ gm, const Buffers<T>& B, const uint8_t* __restrict__ mask) {
   extern __shared__ __align__(32) unsigned char smem[];
   const Model<T>& md = stage_model(gm, smem);
   int gid = blockIdx.x * blockDim.x + threadIdx.x;
@@ -145,7 +177,17 @@ __global__ void __launch_bounds__(128) b2q_settle_kernel(Cfg<T> cf, const Model<
   if (mask && !mask[env]) valid = false;
   T* scr0 = reinterpret_cast<T*>(smem + ((sizeof(Model<T>) + 31) & ~size_t(31))) + (size_t)(blockDim.x >> 2) * (OBS_DIM + INFO_DIM);
   WarpComm cm{(int)(threadIdx.x & 3), reinterpret_cast<unsigned char*>(scr0 + (size_t)(threadIdx.x >> 2) * scratch_floats(FEAT))};
-  settle_lane<T, FEAT>(cm, cf, md, B, env, valid);
+  if constexpr (TILES != 0) settle_lane<T, FEAT>(cm, env_cfg<T, TILES>(cf, tl, env), md, B, env, valid);
+  else settle_lane<T, FEAT>(cm, cf, md, B, env, valid);
+}
+
+template <typename T, int FEAT>
+__global__ void __launch_bounds__(128) b2q_settle_kernel(Cfg<T> cf, const Model<T>* __restrict__ gm, Buffers<T> B, const uint8_t* __restrict__ mask) {
+  settle_cta<T, FEAT, 0>(cf, Tiles{nullptr, 0}, gm, B, mask);
+}
+template <typename T, int FEAT>
+__global__ void __launch_bounds__(128) b2q_settle_tiles_kernel(Cfg<T> cf, Tiles tl, const Model<T>* __restrict__ gm, Buffers<T> B, const uint8_t* __restrict__ mask) {
+  settle_cta<T, FEAT, 1>(cf, tl, gm, B, mask);
 }
 
 template <typename T>
@@ -262,6 +304,7 @@ struct EnvBase {
   virtual int64_t snapshot_bytes() const = 0;
   virtual int snapshot_save(void* dst, cudaStream_t s) = 0;
   virtual int snapshot_load(const void* src, cudaStream_t s) = 0;
+  virtual int set_tiles(const double* tiles, int n_tiles, const int32_t* tile_of_env, cudaStream_t s) = 0;
 };
 
 #define CK(call)                                                                      \
@@ -290,6 +333,8 @@ struct EnvT : EnvBase {
     if (d_model) cudaFree(d_model);
     if (d_def48) cudaFree(d_def48);
     if (d_hf) cudaFree(d_hf);
+    if (d_tiles) cudaFree(d_tiles);
+    if (tl.tile_of_env) cudaFree(const_cast<int32_t*>(tl.tile_of_env));
     if (st_act) cudaFree(st_act);
     if (h_flag) cudaFreeHost(h_flag);
     if (h_snap) cudaFreeHost(h_snap);
@@ -376,7 +421,12 @@ struct EnvT : EnvBase {
       err = buf;
       return B2Q_EINVAL;
     }
-    if (feat) b2q_settle_kernel<T, 1><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, d_model, B, mask);
+    return settle(mask, s);
+  }
+  int settle(const uint8_t* mask, cudaStream_t s) {
+    if (n_tiles && feat) b2q_settle_tiles_kernel<T, 1><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, tl, d_model, B, mask);
+    else if (n_tiles) b2q_settle_tiles_kernel<T, 0><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, tl, d_model, B, mask);
+    else if (feat) b2q_settle_kernel<T, 1><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, d_model, B, mask);
     else b2q_settle_kernel<T, 0><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, d_model, B, mask);
     launches += 1;
     CK(cudaGetLastError());
@@ -404,7 +454,11 @@ struct EnvT : EnvBase {
   int step(const void* action, int donef, void* obs, void* rew, uint8_t* done, void* info, cudaStream_t s) override {
     if (!action || !obs || !rew || !done || !info) { err = "b2q_step: null device pointer"; return B2Q_EINVAL; }
     { int cur = -1; if (cudaGetDevice(&cur) != cudaSuccess || cur != cfg.device) CK(cudaSetDevice(cfg.device)); }   // handles are per GPU
-    if (feat) b2q_step_kernel<T, 1><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, d_model, B, (const T*)action, donef, cfg.auto_reset, (T*)obs, (T*)rew, done, (T*)info);
+    if (n_tiles && feat)
+      b2q_step_tiles_kernel<T, 1><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, tl, d_model, B, (const T*)action, donef, cfg.auto_reset, (T*)obs, (T*)rew, done, (T*)info);
+    else if (n_tiles)
+      b2q_step_tiles_kernel<T, 0><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, tl, d_model, B, (const T*)action, donef, cfg.auto_reset, (T*)obs, (T*)rew, done, (T*)info);
+    else if (feat) b2q_step_kernel<T, 1><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, d_model, B, (const T*)action, donef, cfg.auto_reset, (T*)obs, (T*)rew, done, (T*)info);
     else b2q_step_kernel<T, 0><<<grid_lanes(), tpb, smem_bytes(), s>>>(kc, d_model, B, (const T*)action, donef, cfg.auto_reset, (T*)obs, (T*)rew, done, (T*)info);
     launches++;
     CK(cudaGetLastError());
@@ -498,6 +552,7 @@ struct EnvT : EnvBase {
     return h;
   }
   int snapshot_save(void* dst, cudaStream_t s) override {
+    if (n_tiles) { err = "b2q_snapshot_save: not on a terrain-atlas handle (the snapshot header hashes one height field)"; return B2Q_EINVAL; }
     if (!dst || ((size_t)dst & 15)) { err = "b2q_snapshot_save: dst must be a 16-byte aligned device pointer"; return B2Q_EINVAL; }
     CK(cudaSetDevice(cfg.device));
     CK(b2q_snap::write_header(snap_header(), dst, s));
@@ -506,6 +561,7 @@ struct EnvT : EnvBase {
     return B2Q_OK;
   }
   int snapshot_load(const void* src, cudaStream_t s) override {
+    if (n_tiles) { err = "b2q_snapshot_load: not on a terrain-atlas handle (the snapshot header hashes one height field)"; return B2Q_EINVAL; }
     if (!src || ((size_t)src & 15)) { err = "b2q_snapshot_load: src must be a 16-byte aligned device pointer"; return B2Q_EINVAL; }
     CK(cudaSetDevice(cfg.device));
     // the refusal is a return code, so the header has to reach the host first: one small copy, waited for
@@ -528,6 +584,7 @@ struct EnvT : EnvBase {
   }
   int render(const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int W, int H, uint8_t* rgba, float* depth,
              int32_t* seg, cudaStream_t s) override {
+    if (n_tiles) { err = "b2q_render: not on a terrain-atlas handle (the renderer ray-casts the handle's one height field)"; return B2Q_EINVAL; }
     if (!state || !env_ids || !view || !proj) { err = "b2q_render: null state, env_ids, view or proj"; return B2Q_EINVAL; }
     if (V < 1 || V > 65535) { err = "b2q_render: V must be in [1, 65535]"; return B2Q_EINVAL; }
     if (W < 1 || H < 1 || W > 16384 || H > 16384) { err = "b2q_render: width and height must be in [1, 16384]"; return B2Q_EINVAL; }
@@ -542,6 +599,56 @@ struct EnvT : EnvBase {
     CK(render_launch<T>(a, V, s));
     launches++;
     return B2Q_OK;
+  }
+  // terrain atlas: n_tiles > 0 once b2q_set_terrain_tiles succeeded; kc.hf then points at d_tiles
+  T* d_tiles = nullptr;
+  Tiles tl{nullptr, 0};
+  int n_tiles = 0;
+  int set_tiles(const double* tiles, int nt, const int32_t* tile_of_env, cudaStream_t s) override {
+    if (cfg.terrain_type != 1) { err = "b2q_set_terrain_tiles: needs a height-field handle (terrain_type 1): its hf_* fields give the tiles' grid"; return B2Q_EINVAL; }
+    if (!tiles || !tile_of_env) { err = "b2q_set_terrain_tiles: null tiles or tile_of_env"; return B2Q_EINVAL; }
+    if (nt < 1) { err = "b2q_set_terrain_tiles: n_tiles must be >= 1"; return B2Q_EINVAL; }
+    for (int i = 0; i < B.N; i++) {
+      if (tile_of_env[i] < 0 || tile_of_env[i] >= nt) {
+        char buf[160];
+        snprintf(buf, sizeof buf, "b2q_set_terrain_tiles: tile_of_env[%d] = %d is outside [0, %d)", i, (int)tile_of_env[i], nt);
+        err = buf;
+        return B2Q_EINVAL;
+      }
+    }
+    CK(cudaSetDevice(cfg.device));
+    const size_t per = (size_t)cfg.hf_nx * cfg.hf_ny, n = per * (size_t)nt;   // the kernels offset by tile * per in 64 bits
+    T* tmp = (T*)malloc(n * sizeof(T));
+    if (!tmp) { err = "b2q_set_terrain_tiles: host alloc failed"; return B2Q_ENOMEM; }
+    for (size_t i = 0; i < n; i++) tmp[i] = (T)tiles[i];
+    CK(cudaStreamSynchronize(s));   // the previous atlas may still be read by launches on the stream
+    if (d_tiles) { cudaFree(d_tiles); d_tiles = nullptr; }
+    if (tl.tile_of_env) { cudaFree(const_cast<int32_t*>(tl.tile_of_env)); tl.tile_of_env = nullptr; }
+    n_tiles = 0; kc.hf = d_hf;
+    int32_t* d_map = nullptr;
+    cudaError_t e1 = cudaMalloc(&d_tiles, n * sizeof(T));
+    if (e1 == cudaSuccess) e1 = cudaMemcpy(d_tiles, tmp, n * sizeof(T), cudaMemcpyHostToDevice);
+    free(tmp);
+    if (e1 == cudaSuccess) e1 = cudaMalloc(&d_map, (size_t)B.N * sizeof(int32_t));
+    if (e1 == cudaSuccess) e1 = cudaMemcpy(d_map, tile_of_env, (size_t)B.N * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (e1 != cudaSuccess) {
+      if (d_tiles) cudaFree(d_tiles);
+      if (d_map) cudaFree(d_map);
+      d_tiles = nullptr;
+      CK(e1);
+    }
+    if (smem_bytes() > 48 * 1024) {
+      if (feat) {
+        CK(cudaFuncSetAttribute(b2q_step_tiles_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+        CK(cudaFuncSetAttribute(b2q_settle_tiles_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+      } else {
+        CK(cudaFuncSetAttribute(b2q_step_tiles_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+        CK(cudaFuncSetAttribute(b2q_settle_tiles_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+      }
+    }
+    tl.tile_of_env = d_map; tl.tile_elems = (long long)per;
+    n_tiles = nt; kc.hf = d_tiles;
+    return settle(nullptr, s);   // every env's reset snapshot, settled on its own tile with the dynamics it has
   }
 };
 
@@ -614,6 +721,9 @@ int b2q_set_max_episode_steps(B2QHandle h, int m) {
 int64_t b2q_snapshot_bytes(B2QHandle h) { return h ? h->impl->snapshot_bytes() : B2Q_EINVAL; }
 int b2q_snapshot_save(B2QHandle h, void* dst, void* s) { return h ? h->impl->snapshot_save(dst, (cudaStream_t)s) : B2Q_EINVAL; }
 int b2q_snapshot_load(B2QHandle h, const void* src, void* s) { return h ? h->impl->snapshot_load(src, (cudaStream_t)s) : B2Q_EINVAL; }
+int b2q_set_terrain_tiles(B2QHandle h, const double* tiles_host, int n_tiles, const int32_t* tile_of_env, void* stream) {
+  return h ? h->impl->set_tiles(tiles_host, n_tiles, tile_of_env, (cudaStream_t)stream) : B2Q_EINVAL;
+}
 int b2q_render(B2QHandle h, const void* state, const int32_t* env_ids, int V, const float* view, const float* proj, int width, int height, uint8_t* rgba,
                float* depth, int32_t* seg, void* stream) {
   return h ? h->impl->render(state, env_ids, V, view, proj, width, height, rgba, depth, seg, (cudaStream_t)stream) : B2Q_EINVAL;

@@ -42,6 +42,7 @@ class VecQuadrupedalEnv:
         self.lib.b2q_default_config(C.byref(c))
         c.num_envs, c.device, c.precision, c.auto_reset = self.num_envs, int(device), 0 if self.dtype == torch.float32 else 1, int(auto_reset)
         self._hf_keep = None
+        self.n_tiles = 0            # > 0 once set_terrain_tiles made this a terrain-atlas env
         if heightfield is not None:
             hf, x0, y0, cell = heightfield
             hf = np.ascontiguousarray(hf, dtype=np.float64)
@@ -130,9 +131,30 @@ class VecQuadrupedalEnv:
         _check(self.lib, self.h, self.lib.b2q_set_max_episode_steps(self.h, int(m)), "b2q_set_max_episode_steps")
         self.cfg.max_episode_steps = int(m)
 
+    def set_terrain_tiles(self, tiles, tile_of_env):
+        """Terrain atlas (b2q_set_terrain_tiles): env i reads the height field tiles[tile_of_env[i]] from now on.  tiles: [T, ny, nx] on this
+        env's height-field grid (make_terrain_tiles gives such a stack), tile_of_env: [N] indices in [0, T).  Every env's reset snapshot is
+        settled again on its tile with the dynamics it has; call reset() before the next step.  An atlas env has no state_dict,
+        load_state_dict or get_camera_image."""
+        if self.cfg.terrain_type != 1:
+            raise ValueError("set_terrain_tiles needs an env built on a height field: the tiles share its grid")
+        t = np.ascontiguousarray(tiles, dtype=np.float64)
+        if t.ndim != 3 or t.shape[1:] != (self.cfg.hf_ny, self.cfg.hf_nx):
+            raise ValueError("tiles of shape %s, this env's grid needs [T, %d, %d]" % (list(t.shape), self.cfg.hf_ny, self.cfg.hf_nx))
+        m = np.ascontiguousarray(tile_of_env, dtype=np.int32).reshape(-1)
+        if m.shape[0] != self.num_envs:
+            raise ValueError("tile_of_env has %d entries for %d envs" % (m.shape[0], self.num_envs))
+        _check(self.lib, self.h, self.lib.b2q_set_terrain_tiles(self.h, t.ctypes.data, int(t.shape[0]), m.ctypes.data, self._stream()), "b2q_set_terrain_tiles")
+        self.n_tiles = int(t.shape[0])
+
+    def _refuse_atlas(self, what):
+        if self.n_tiles:
+            raise RuntimeError("%s: not on a terrain-atlas env (set_terrain_tiles): the snapshot and the camera know one height field" % what)
+
     def state_dict(self):
         """Everything a later step or reset reads (b2q_snapshot_save: the device pool and the episode step limit), plus the last step's
         outputs, as CPU tensors."""
+        self._refuse_atlas("state_dict")
         blob = torch.empty(int(self.lib.b2q_snapshot_bytes(self.h)), dtype=torch.uint8, device=self.device)
         _check(self.lib, self.h, self.lib.b2q_snapshot_save(self.h, blob.data_ptr(), self._stream()), "b2q_snapshot_save")
         return {"snapshot": blob.cpu(), "max_episode_steps": int(self.cfg.max_episode_steps), "obs": self.obs.cpu(), "reward": self.reward.cpu(),
@@ -141,6 +163,7 @@ class VecQuadrupedalEnv:
     def load_state_dict(self, sd):
         """Restores a state_dict() of an env built with the same configuration; raises ValueError for a blob of another size and
         RuntimeError (naming the first differing field) for one of another configuration."""
+        self._refuse_atlas("load_state_dict")
         want = int(self.lib.b2q_snapshot_bytes(self.h))
         blob = sd["snapshot"]
         if blob.dtype != torch.uint8 or blob.numel() != want:
@@ -158,6 +181,7 @@ class VecQuadrupedalEnv:
         camera of each env (render.follow_camera).  Returns device tensors (rgba [V,H,W,4] uint8, depth [V,H,W] float32 OpenGL
         depth-buffer values, seg [V,H,W] int32), which the next call with the same sizes overwrites: the buffers are reused, so the
         call can be captured in a CUDA graph (pass env_ids / view / proj as device tensors or None there)."""
+        self._refuse_atlas("get_camera_image")
         from . import render
         dev, W, H = self.device, int(width), int(height)
         if env_ids is None:

@@ -87,6 +87,41 @@ def make_terrain(task, step_height=0.08, step_width=0.3, slope=0.3, n_steps=5, a
     return _profile_to_field(xs, h1 + h2, cell)
 
 
+# the grid values each task's make_terrain reads: stairs use the height and width, ramps the slope (and the rise, from the height)
+GRID_KEYS = {"stairstair": ("step_height", "step_width"), "stairslope": ("step_height", "step_width", "slope"),
+             "slopestair": ("step_height", "step_width", "slope"), "slopeslope": ("step_height", "slope")}
+_GRID_VALUES = {"step_height": STEP_HEIGHT, "step_width": STEP_WIDTH, "slope": SLOPE}
+
+
+def terrain_grid(task):
+    """Every geometry of the reference's grids (train.py:48-50) that make_terrain(task) distinguishes, as make_terrain keyword dicts in
+    row-major order of GRID_KEYS[task]: 88 for stairstair, 968 for stairslope and slopestair, 121 for slopeslope.  Raises ValueError for
+    a task without such a grid (ground, plane, balancebeam, terrain)."""
+    if task not in GRID_KEYS:
+        raise ValueError("task %r has no terrain grid: its terrain does not depend on the step height, width or slope (grids exist for %s)"
+                         % (task, ", ".join(GRID_KEYS)))
+    keys = GRID_KEYS[task]
+    return [dict(zip(keys, (float(v) for v in vals))) for vals in np.stack(np.meshgrid(*(_GRID_VALUES[k] for k in keys), indexing="ij"), -1).reshape(-1, len(keys))]
+
+
+def make_terrain_tiles(task, geoms, step_y=0.05):
+    """The height fields of `geoms` (make_terrain keyword dicts) on one grid: (tiles [T, ny, nx], x0, y0, cell), the arguments of
+    VecQuadrupedalEnv.set_terrain_tiles.  The fields share x0, y0, cell and ny and differ in length; each shorter one is padded to the
+    longest with copies of its last column.  Every preset ends in a flat run-out and the kernel clamps a lookup at the field's edge, so a
+    padded tile gives the heights and normals of its unpadded field wherever the robot can stand."""
+    fields = [make_terrain(task, step_y=step_y, **g) for g in geoms]
+    if not fields or any(f is None for f in fields):
+        raise ValueError("make_terrain_tiles needs at least one geometry of a height-field task, got %d for %r" % (len(fields), task))
+    _, x0, y0, cell = fields[0]
+    nx = max(f[0].shape[1] for f in fields)
+    tiles = np.empty((len(fields), fields[0][0].shape[0], nx), dtype=np.float64)
+    for t, (hf, fx0, fy0, fcell) in enumerate(fields):
+        assert (fx0, fy0, fcell, hf.shape[0]) == (x0, y0, cell, tiles.shape[1])
+        tiles[t, :, :hf.shape[1]] = hf
+        tiles[t, :, hf.shape[1]:] = hf[:, -1:]
+    return tiles, x0, y0, cell
+
+
 def sample_terrain_params(rng):
     """One draw of the reference's per-run terrain parameters (train.py:48-50)."""
     return dict(step_height=float(rng.choice(STEP_HEIGHT)), slope=float(rng.choice(SLOPE)), step_width=float(rng.choice(STEP_WIDTH)))

@@ -34,7 +34,7 @@ from .es import PopulationEvaluator, SimpleGA, TrainEpisodeStats, solutions_to_e
 from .etg import ETG_layer, Opt_with_points
 from .replay import ReplayMemory
 from .run_state import write_atomic
-from .terrain import make_terrain
+from .terrain import GRID_KEYS, make_terrain, make_terrain_tiles, terrain_grid
 
 GAMMA, TAU, ALPHA, ACTOR_LR, CRITIC_LR = 0.99, 0.005, 0.2, 3e-4, 3e-4     # train.py:43-47
 
@@ -75,6 +75,7 @@ def parser():
     p.add_argument("--load", type=str, default="", help="itr_*.pt to restore the agent from (and the .npz next to it for w, b, param)")
     p.add_argument("--eval", type=int, default=0, help="1: evaluate the --load checkpoint instead of training (run_evaluate_episodes, train.py:182-211,438-449)")
     p.add_argument("--eval_envs", type=int, default=1, help="envs of the --eval episode (one episode each, no auto-reset)")
+    p.add_argument("--terrain_grid", type=int, default=0, help=TERRAIN_GRID_HELP)
     p.add_argument("--render_dir", type=str, default="", help="--eval: write env 0's camera image of every step to DIR/img{step}.png (train.py:196-199); empty = no frames")
     p.add_argument("--render_width", type=int, default=640)
     p.add_argument("--render_height", type=int, default=480)
@@ -149,6 +150,10 @@ def obs_width(args):
 
 def check_args(p, args):
     """The argument errors of main, raised (p.error) before any device work."""
+    check_terrain_grid(p, args)
+    if getattr(args, "terrain_grid", 0) and args.sensor_noise:
+        p.error("--terrain_grid 1 with --sensor_noise 1: the step kernel keys its sensor noise by the env's index in the handle, so a "
+                "geometry's envs would not draw the noise of the same --eval 1 episode")
     if args.ES and not args.ETG:
         p.error("--ETG 0 with --ES 1: the ES phase searches the ETG, which --ETG 0 turns off")
     if args.train_eval_envs < 0 or args.e_step_growth < 0:
@@ -558,7 +563,8 @@ def run_evaluate_episodes(env, w, b, policy=None, act_bound=0.3, max_step=EVAL_M
     noise by it); None = zero residual (the open-loop ETG).  x_offset: [N] start displacements along x for env.reset (bctrain --x_noise 1).
     Each env's return, length, EVAL_TERMS sums and velx success count freeze at its first done, all in one b2q_es_accumulate_terms launch
     per step.  render(steps): per-step hook.
-    Returns {mean_return, mean_length, terms: {term: mean episode sum}, success_rate: mean over envs of count / length}."""
+    Returns {mean_return, mean_length, terms: {term: mean episode sum}, success_rate: mean over envs of count / length, per_env}, per_env
+    holding the [N] device tensors these means are taken over: {return, length, terms: {term: episode sum}, success_rate}."""
     from . import _lib
     from .es import EpisodeStats
     n = env.num_envs
@@ -576,7 +582,55 @@ def run_evaluate_episodes(env, w, b, policy=None, act_bound=0.3, max_step=EVAL_M
             break
     return {"mean_return": float(stats.ret.double().mean()), "mean_length": float(stats.len.double().mean()),
             "terms": {k: float(stats.term_sum[j].double().mean()) for j, k in enumerate(EVAL_TERMS)},
-            "success_rate": float(stats.success_rate().double().mean())}
+            "success_rate": float(stats.success_rate().double().mean()),
+            "per_env": {"return": stats.ret, "length": stats.len, "terms": {k: stats.term_sum[j] for j, k in enumerate(EVAL_TERMS)},
+                        "success_rate": stats.success_rate()}}
+
+
+TERRAIN_GRID_HELP = ("--eval 1: score on every stair / slope geometry of the task's grid (terrain.terrain_grid: train.py:48-50's step heights, "
+                     "widths and slopes) in one batched rollout of --eval_envs envs per geometry; one JSON line per geometry and a summary")
+
+
+def check_terrain_grid(p, args):
+    """The argument errors of --terrain_grid 1 (train, pretrain, bctrain), raised (p.error) before any device work."""
+    if not getattr(args, "terrain_grid", 0):
+        return
+    if not args.eval:
+        p.error("--terrain_grid 1 scores a checkpoint or gait on every geometry of the task's grid: it needs --eval 1")
+    if args.render_dir:
+        p.error("--terrain_grid 1 with --render_dir: the camera ray-casts one height field, and a grid evaluation steps one per geometry")
+    if args.task_mode not in GRID_KEYS:
+        p.error("--terrain_grid 1 with --task_mode %s: this terrain has no step height, width or slope to vary (grids exist for %s)"
+                % (args.task_mode, ", ".join(GRID_KEYS)))
+
+
+def evaluate_terrain_grid(args, env_cfg, w, b, policy=None, act_bound=0.3, max_step=EVAL_MAX_STEP, x_offset=None):
+    """--eval 1 --terrain_grid 1 of train, pretrain and bctrain: the --eval 1 episode of --eval_envs envs on every geometry of
+    terrain_grid(--task_mode), all in one terrain-atlas env (env g * eval_envs + j runs env j of geometry g), with env_cfg's
+    configuration and the --dynamic_param dynamics.  policy(obs, steps) sees every geometry's rows at once; x_offset: [eval_envs] start
+    offsets, the same for every geometry.  Prints one JSON line per geometry (its grid values and run_evaluate_episodes' record over its
+    envs, taken as run_evaluate_episodes takes it) and a summary line; returns those records."""
+    geoms = terrain_grid(args.task_mode)
+    tiles, x0, y0, cell = make_terrain_tiles(args.task_mode, geoms, args.step_y)
+    n, G = args.eval_envs, len(geoms)
+    env = make_eval_env(args, dict(env_cfg, heightfield=(tiles[0], x0, y0, cell)), n * G)
+    env.set_terrain_tiles(tiles, np.repeat(np.arange(G, dtype=np.int32), n))
+    del tiles
+    r = run_evaluate_episodes(env, w, b, policy=policy, act_bound=act_bound, max_step=max_step, x_offset=None if x_offset is None else np.tile(x_offset, G))
+    pe = r["per_env"]
+    cols = [pe["return"], pe["length"], pe["success_rate"]] + [pe["terms"][k] for k in EVAL_TERMS]
+    means = torch.stack([torch.stack([c[g * n:(g + 1) * n].double().mean() for c in cols]) for g in range(G)]).tolist()
+    env.close()
+    recs = []
+    for geom, m in zip(geoms, means):
+        rec = dict(geom, mean_return=m[0], mean_length=m[1], success_rate=m[2], terms={k: m[3 + j] for j, k in enumerate(EVAL_TERMS)})
+        recs.append(rec)
+        print(json.dumps(rec), flush=True)
+    worst = min(range(G), key=lambda g: recs[g]["mean_return"])
+    summary = {"geometries": G, "eval_envs": n, "task_mode": args.task_mode, "mean_return": float(np.mean([rc["mean_return"] for rc in recs])),
+               "worst": geoms[worst], "worst_return": recs[worst]["mean_return"]}
+    print(json.dumps(summary), flush=True)
+    return recs + [summary]
 
 
 def frame_writer(env, args):
@@ -592,13 +646,18 @@ def frame_writer(env, args):
 
 def evaluate(args, env_cfg, act_bound):
     """--eval 1: one deterministic episode per env of the restored agent and ETG (w, b) on the training env's config, at most
-    EVAL_MAX_STEP + 1 control steps (run_evaluate_episodes).  Prints and returns one JSON record."""
+    EVAL_MAX_STEP + 1 control steps (run_evaluate_episodes).  Prints and returns one JSON record; with --terrain_grid 1, the records of
+    evaluate_terrain_grid."""
     n = args.eval_envs
+    z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
+    w, b = z["w"], z["b"]
+    if args.terrain_grid:
+        agent = MujocoAgent(obs_width(args), 12, seed=args.seed)
+        agent.restore(args.load)
+        return evaluate_terrain_grid(args, env_cfg, w, b, policy=lambda o, s: agent.predict_batch(o), act_bound=act_bound, max_step=EVAL_MAX_STEP)
     env = make_eval_env(args, env_cfg, n)
     agent = MujocoAgent(env.observation_dim, 12, seed=args.seed)
     agent.restore(args.load)
-    z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
-    w, b = z["w"], z["b"]
     r = run_evaluate_episodes(env, w, b, policy=lambda o, s: agent.predict_batch(o), act_bound=act_bound, max_step=EVAL_MAX_STEP,
                               render=frame_writer(env, args) if args.render_dir else None)
     rec = {"eval_envs": n, "mean_return": r["mean_return"], "mean_length": r["mean_length"], "terms": r["terms"]}
