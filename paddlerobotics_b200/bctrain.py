@@ -25,7 +25,9 @@ import torch
 from . import bc
 from .agent import MujocoAgent, SACLearner
 from .env import VecQuadrupedalEnv, apply_dynamic_param, etg_of_path, quadrupedal_config
-from .train import TERRAIN_GRID_HELP, check_terrain_grid, evaluate_terrain_grid, frame_writer, run_evaluate_episodes
+from .dynamics_grid import HELP as DYNAMICS_GRID_HELP
+from .train import (TERRAIN_GRID_HELP, check_dynamics_grid, check_terrain_grid, evaluate_dynamics_grid, evaluate_terrain_grid, frame_writer,
+                    run_evaluate_episodes)
 
 ACTOR_LR, CRITIC_LR = 3e-4, 3e-4            # BCtrain.py:44-45
 EVAL_STEPS, RANDOM_EVAL_STEPS = 600, 800    # run_evaluate_episodes(agent, env, 600, ...) BCtrain.py:321; run_random_eval(..., 800, ...) :302
@@ -82,6 +84,7 @@ def parser():
     p.add_argument("--eval_every_steps", type=float, default=1e4)             # EVAL_EVERY_STEPS
     p.add_argument("--eval_envs", type=int, default=1, help="envs of each evaluation episode (one episode each, no auto-reset)")
     p.add_argument("--terrain_grid", type=int, default=0, help=TERRAIN_GRID_HELP)
+    p.add_argument("--dynamics_grid", type=int, default=0, help=DYNAMICS_GRID_HELP)
     p.add_argument("--graph_steps", type=int, default=64, help="BC updates per captured CUDA graph")
     p.add_argument("--seed", type=int, default=0)
     p.add_argument("--render_dir", type=str, default="", help="--eval 1: write env 0's camera image of every step to DIR/img{step}.png")
@@ -179,6 +182,7 @@ def main(argv=None):
         p.error("--save_state 1 writes <outdir>/<suffix>/state.pt: it needs --outdir")
     check_supported(args)
     check_terrain_grid(p, args)
+    check_dynamics_grid(p, args)
     torch.manual_seed(args.seed); np.random.seed(args.seed)
     # a resume takes the gait and the expert from the state, not from --ETG_path / --ref_agent, whose files may have changed since
     w, b = etg_of_path(args.ETG_path, args.ETG_T) if state is None else (state["w"], state["b"])
@@ -290,9 +294,10 @@ def random_eval(args, learner, expert, env, w, b, bound):
 
 def evaluate(args, student, w, b, bound):
     """--eval 1 --load X.pt: run_evaluate_episodes (BCtrain.py:147-176,317-326) — the student's deterministic episode, at most 600 steps, on
-    its (noisy) obs[3:]; one JSON line; --render_dir writes img{step}.png of env 0.  With --terrain_grid 1, the records of
-    train.evaluate_terrain_grid, in which every geometry's envs see the sensor noise and --x_noise offsets of this episode."""
-    if args.terrain_grid:
+    its (noisy) obs[3:]; one JSON line; --render_dir writes img{step}.png of env 0.  With --terrain_grid 1 or --dynamics_grid 1, the
+    records of train.evaluate_terrain_grid or evaluate_dynamics_grid, in which every setting's envs see the sensor noise and --x_noise
+    offsets of this episode."""
+    if args.terrain_grid or getattr(args, "dynamics_grid", 0):
         return evaluate_grid(args, student, w, b, bound)
     env = make_vec_env(args, args.eval_envs, auto_reset=False)
     obs_mem = bc.BCReplayMemory(1, 46, 49, device=env.device)
@@ -306,9 +311,10 @@ def evaluate(args, student, w, b, bound):
 
 
 def evaluate_grid(args, student, w, b, bound):
-    """--eval 1 --terrain_grid 1.  b2q_bc_observe keys the student's noise by the observation row, so the noise of env j of a
-    single-terrain episode is drawn once per step on zero rows (0 + sigma * normal is the noise itself) and added to env j of every
-    geometry: the same float32 sum the kernel forms, so each geometry's student sees that episode's observations."""
+    """--eval 1 with --terrain_grid 1 or --dynamics_grid 1.  b2q_bc_observe keys the student's noise by the observation row, so the noise
+    of env j of a single-setting episode is drawn once per step on zero rows (0 + sigma * normal is the noise itself) and added to env j
+    of every geometry or dynamics setting: the same float32 sum the kernel forms, so each setting's student sees that episode's
+    observations."""
     n, noise = args.eval_envs, bool(args.sensor_noise)
     xo = np.random.uniform(-0.1, 0.1, n) if args.x_noise else None
     obs_mem = bc.BCReplayMemory(1, 46, 49, device="cuda")
@@ -319,7 +325,8 @@ def evaluate_grid(args, student, w, b, bound):
             return student.predict_batch(obs_mem.observe(o, s, noise=False, append=False, seed=args.seed))
         z = obs_mem.observe(zero, s, noise=True, append=False, seed=args.seed)
         return student.predict_batch((o[:, 3:].reshape(-1, n, 46) + z).reshape(-1, 46))
-    return evaluate_terrain_grid(args, env_kwargs(args), w, b, policy=policy, act_bound=bound, max_step=EVAL_STEPS, x_offset=xo)
+    grid = evaluate_terrain_grid if args.terrain_grid else evaluate_dynamics_grid
+    return grid(args, env_kwargs(args), w, b, policy=policy, act_bound=bound, max_step=EVAL_STEPS, x_offset=xo)
 
 
 if __name__ == "__main__":

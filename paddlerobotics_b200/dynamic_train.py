@@ -17,6 +17,7 @@ starts from zeros.  --alg cma is refused: the reference's set_solver has no cma 
     python -m paddlerobotics_b200.dynamic_train --data_dir data/dynamic --alg ga --steps 10000
     python -m paddlerobotics_b200.dynamic_train --data_dir data/dynamic --save_state 1; python -m paddlerobotics_b200.dynamic_train --resume Dynamic/exp0/state.pt --steps N
     python -m paddlerobotics_b200.dynamic_train --eval 1 --load Dynamic/exp0/dynamic_param9027.npy
+    python -m paddlerobotics_b200.dynamic_train --eval 1 --load Dynamic/exp0/dynamic_param9027.npy --dynamics_grid 1   # the landscape around it
     python -m paddlerobotics_b200.train --dynamic_param Dynamic/exp0/dynamic_param9027.npy     # train the expert on the result
 """
 import argparse
@@ -44,6 +45,9 @@ def parser():
     p.add_argument("--K", type=int, default=20, help="individuals per actor")
     p.add_argument("--load", type=str, default="", help="dynamic_param*.npy to evaluate with --eval 1 (training always starts from zeros)")
     p.add_argument("--eval", type=int, default=0, help="1: evaluate the --load vector on the height table")
+    p.add_argument("--dynamics_grid", type=int, default=0, help="--eval 1: the identification landscape around the --load vector: each group of "
+                   "its 48 parameters set alone to -1, -0.75, ..., 1, all 82 vectors scored in one batch on the height table (eval_reward) and "
+                   "on the exp and ori tables (train_reward); one JSON line per vector and a summary")
     p.add_argument("--suffix", type=str, default="exp0")
     p.add_argument("--sigma", type=float, default=0.1)
     p.add_argument("--gamma", type=float, default=1, help="accepted and ignored, as in the reference")
@@ -129,6 +133,8 @@ def main(argv=None):
         p.error("--alg %s is not provided (the reference's set_solver has no %s branch); supported algorithms: %s" % (args.alg, args.alg, ", ".join(ALGS)))
     if args.eval and not args.load:
         p.error("--eval 1 evaluates a dynamics vector: it needs --load dynamic_param*.npy")
+    if getattr(args, "dynamics_grid", 0) and not args.eval:          # a state file may predate the flag
+        p.error("--dynamics_grid 1 evaluates the landscape around a dynamics vector: it needs --eval 1 --load dynamic_param*.npy")
     try:
         gait, mean_dict = load_data(args.data_dir)
     except ValueError as e:
@@ -160,6 +166,8 @@ def run(args, gait, mean_dict, rank, world, local, state=None):
     cfg = evaluator_config()
     if args.eval and rank != 0:
         return []
+    if args.eval and args.dynamics_grid:
+        return landscape(args, gait, mean_dict, cfg, local)
     height = DynamicsEvaluator(1, gait, mean_dict, keys=("height",), steps=STEPS, device=local, **cfg) if rank == 0 else None
 
     def eval_height(param):
@@ -201,6 +209,36 @@ def run(args, gait, mean_dict, rank, world, local, state=None):
     if height is not None:
         height.env.close()
     return log
+
+
+COPIES = 8      # envs per vector and table in the landscape: one warp of the step kernel
+
+
+def landscape(args, gait, mean_dict, cfg, device=0):
+    """--eval 1 --load P.npy --dynamics_grid 1: the 82 vectors of dynamics_grid.swept_params(P) (P, then P with one group set to each
+    level), scored in one batch by a DynamicsEvaluator on `height` (eval_reward, what --eval 1 reports) and one on `exp` and `ori`
+    (train_reward, what the epochs maximise).  Every vector fills whole warps (COPIES envs per table): the evaluators' configuration has
+    joint limits and knee contacts, whose general contact solve the step kernel switches per warp of 8 robots, so no other vector's
+    robots can switch a vector's solve: its eval_reward is what --eval 1 --load of it reports (DESIGN §8i).  Prints one JSON line per vector and a summary: the centre's rewards and, per
+    group, the level with the best train_reward and the range of train_reward over the levels (a flat group is one the data does not
+    identify), most sensitive group first."""
+    from . import dynamics_grid
+    from .es import DynamicsEvaluator
+    sols = np.repeat(dynamics_grid.swept_params(np.load(args.load).reshape(-1)), COPIES, 0)
+    rewards = {}
+    for name, keys in (("eval_reward", ("height",)), ("train_reward", ("exp", "ori"))):
+        ev = DynamicsEvaluator(len(sols), gait, mean_dict, keys=keys, steps=STEPS, device=device, **cfg)
+        rewards[name] = ev.evaluate(sols).double().cpu().numpy()[::COPIES]
+        ev.env.close()
+    recs = []
+    for s, setting in enumerate(dynamics_grid.setting_records()):
+        rec = dict(setting, eval_reward=float(rewards["eval_reward"][s]), train_reward=float(rewards["train_reward"][s]))
+        recs.append(rec)
+        print(json.dumps(rec), flush=True)
+    summary = {"settings": len(recs), "load": args.load, "centre_eval_reward": recs[0]["eval_reward"], "centre_train_reward": recs[0]["train_reward"],
+               "groups": dynamics_grid.group_summary(recs[1:], "train_reward", highest=True)}
+    print(json.dumps(summary), flush=True)
+    return recs + [summary]
 
 
 if __name__ == "__main__":

@@ -359,9 +359,13 @@ def apply_dynamic_param(env, path):
     """A command's --dynamic_param: PATH.npy holds a 48-vector in [-1, 1] (a dynamic_param{epoch}.npy of dynamic_train) that goes through
     param2dynamic_dict to every env of `env`; an empty path keeps the nominal dynamics.  Returns env."""
     if path:
-        row = dynamic_dict_to_row(param2dynamic_dict(np.load(path).reshape(-1)))
-        env.set_dynamics(np.repeat(row[None], env.num_envs, 0))
+        env.set_dynamics(np.repeat(dynamic_param_row(path)[None], env.num_envs, 0))
     return env
+
+
+def dynamic_param_row(path):
+    """The [48] engine row of a command's --dynamic_param (see apply_dynamic_param): the nominal row when `path` is empty."""
+    return dynamic_dict_to_row(param2dynamic_dict(np.load(path).reshape(-1))) if path else dynamic_dict_to_row()
 
 
 def etg_of_path(ETG_path, ETG_T=0.5):

@@ -42,6 +42,7 @@ SUCCESS_VELX = 0.3          # pretrain.py:147
 
 
 def parser():
+    from .dynamics_grid import HELP as DYNAMICS_GRID_HELP
     from .train import TERRAIN_GRID_HELP
     p = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     # ---- pretrain.py:292-329
@@ -88,6 +89,7 @@ def parser():
     p.add_argument("--eval_every_steps", type=int, default=EVAL_EVERY_STEPS, help="evaluation and itr_*.npz cadence in env steps")
     p.add_argument("--eval_envs", type=int, default=1, help="envs of each evaluation episode (one episode each, no auto-reset)")
     p.add_argument("--terrain_grid", type=int, default=0, help=TERRAIN_GRID_HELP)
+    p.add_argument("--dynamics_grid", type=int, default=0, help=DYNAMICS_GRID_HELP)
     p.add_argument("--dynamic_param", type=str, default="", help="PATH.npy: a 48-vector in [-1, 1] -> param2dynamic_dict -> every env "
                    "(pretrain.py:192-193); empty = nominal dynamics")
     p.add_argument("--seed", type=int, default=0, help="seeds np.random before the solver is built")
@@ -173,8 +175,9 @@ def main(argv=None):
     check_supported(args)
     if args.eval and not args.load:
         p.error("--eval 1 evaluates a gait: it needs --load X.npz")
-    from .train import check_terrain_grid
+    from .train import check_dynamics_grid, check_terrain_grid
     check_terrain_grid(p, args)
+    check_dynamics_grid(p, args)
     if args.popsize < 1 or args.es_rollouts < 1 or args.es_train_steps < 1 or args.eval_every_steps < 1 or args.eval_envs < 1:
         p.error("--popsize, --es_rollouts, --es_train_steps, --eval_every_steps and --eval_envs must be positive")
     if not args.eval and int(args.popsize * 0.1) < 1:
@@ -194,12 +197,15 @@ def make_eval_env(args, cfg, device=0):
 
 def evaluate(args):
     """--eval 1 --load X.npz: the file's (w, b) with the zero residual, one episode per env of --eval_envs, at most 601 steps; one JSON line;
-    --render_dir writes img{step}.png of env 0 for every step taken (pretrain.py:278-289)."""
-    from .train import evaluate_terrain_grid, frame_writer, run_evaluate_episodes
+    --render_dir writes img{step}.png of env 0 for every step taken (pretrain.py:278-289).  --terrain_grid 1 / --dynamics_grid 1: the
+    records of train.evaluate_terrain_grid / evaluate_dynamics_grid."""
+    from .train import evaluate_dynamics_grid, evaluate_terrain_grid, frame_writer, run_evaluate_episodes
     with np.load(args.load) as z:
         w, b = z["w"], z["b"]
     if args.terrain_grid:
         return evaluate_terrain_grid(args, env_config(args), w, b, policy=None, max_step=EVAL_MAX_STEP)
+    if getattr(args, "dynamics_grid", 0):
+        return evaluate_dynamics_grid(args, env_config(args), w, b, policy=None, max_step=EVAL_MAX_STEP)
     env = make_eval_env(args, env_config(args))
     r = run_evaluate_episodes(env, w, b, policy=None, max_step=EVAL_MAX_STEP, render=frame_writer(env, args) if args.render_dir else None)
     rec = {"eval_envs": args.eval_envs, **{k: v for k, v in r.items() if k != "per_env"}}

@@ -27,9 +27,9 @@ import time
 import numpy as np
 import torch
 
-from . import _lib, dist_run, run_state
+from . import _lib, dist_run, dynamics_grid, run_state
 from .agent import MujocoAgent, SACLearner, flatten_params
-from .env import VecQuadrupedalEnv, apply_dynamic_param
+from .env import VecQuadrupedalEnv, apply_dynamic_param, dynamic_param_row
 from .es import PopulationEvaluator, SimpleGA, TrainEpisodeStats, solutions_to_etg_device
 from .etg import ETG_layer, Opt_with_points
 from .replay import ReplayMemory
@@ -76,6 +76,7 @@ def parser():
     p.add_argument("--eval", type=int, default=0, help="1: evaluate the --load checkpoint instead of training (run_evaluate_episodes, train.py:182-211,438-449)")
     p.add_argument("--eval_envs", type=int, default=1, help="envs of the --eval episode (one episode each, no auto-reset)")
     p.add_argument("--terrain_grid", type=int, default=0, help=TERRAIN_GRID_HELP)
+    p.add_argument("--dynamics_grid", type=int, default=0, help=dynamics_grid.HELP)
     p.add_argument("--render_dir", type=str, default="", help="--eval: write env 0's camera image of every step to DIR/img{step}.png (train.py:196-199); empty = no frames")
     p.add_argument("--render_width", type=int, default=640)
     p.add_argument("--render_height", type=int, default=480)
@@ -154,6 +155,10 @@ def check_args(p, args):
     if getattr(args, "terrain_grid", 0) and args.sensor_noise:
         p.error("--terrain_grid 1 with --sensor_noise 1: the step kernel keys its sensor noise by the env's index in the handle, so a "
                 "geometry's envs would not draw the noise of the same --eval 1 episode")
+    check_dynamics_grid(p, args)
+    if getattr(args, "dynamics_grid", 0) and args.sensor_noise:
+        p.error("--dynamics_grid 1 with --sensor_noise 1: the step kernel keys its sensor noise by the env's index in the handle, so a "
+                "setting's envs would not draw the noise of the same --eval 1 episode")
     if args.ES and not args.ETG:
         p.error("--ETG 0 with --ES 1: the ES phase searches the ETG, which --ETG 0 turns off")
     if args.train_eval_envs < 0 or args.e_step_growth < 0:
@@ -604,33 +609,75 @@ def check_terrain_grid(p, args):
                 % (args.task_mode, ", ".join(GRID_KEYS)))
 
 
+def evaluate_settings(env, settings, summary, w, b, policy=None, act_bound=0.3, max_step=EVAL_MAX_STEP, x_offset=None):
+    """The grid evaluations' shared core: the --eval 1 episode of n = env.num_envs / len(settings) envs for every setting, all in `env`,
+    which the caller has set up so that env s * n + j runs env j of setting s.  policy(obs, steps) sees every setting's rows at once;
+    x_offset: [n] start offsets, the same for every setting.  Each setting's record is its dict followed by run_evaluate_episodes' record
+    over its envs, taken as run_evaluate_episodes takes it.  Prints one JSON line per setting, then summary(records); closes env;
+    returns the records and the summary."""
+    S = len(settings)
+    n = env.num_envs // S
+    r = run_evaluate_episodes(env, w, b, policy=policy, act_bound=act_bound, max_step=max_step, x_offset=None if x_offset is None else np.tile(x_offset, S))
+    pe = r["per_env"]
+    cols = [pe["return"], pe["length"], pe["success_rate"]] + [pe["terms"][k] for k in EVAL_TERMS]
+    means = torch.stack([torch.stack([c[s * n:(s + 1) * n].double().mean() for c in cols]) for s in range(S)]).tolist()
+    env.close()
+    recs = []
+    for setting, m in zip(settings, means):
+        rec = dict(setting, mean_return=m[0], mean_length=m[1], success_rate=m[2], terms={k: m[3 + j] for j, k in enumerate(EVAL_TERMS)})
+        recs.append(rec)
+        print(json.dumps(rec), flush=True)
+    summ = summary(recs)
+    print(json.dumps(summ), flush=True)
+    return recs + [summ]
+
+
 def evaluate_terrain_grid(args, env_cfg, w, b, policy=None, act_bound=0.3, max_step=EVAL_MAX_STEP, x_offset=None):
-    """--eval 1 --terrain_grid 1 of train, pretrain and bctrain: the --eval 1 episode of --eval_envs envs on every geometry of
-    terrain_grid(--task_mode), all in one terrain-atlas env (env g * eval_envs + j runs env j of geometry g), with env_cfg's
-    configuration and the --dynamic_param dynamics.  policy(obs, steps) sees every geometry's rows at once; x_offset: [eval_envs] start
-    offsets, the same for every geometry.  Prints one JSON line per geometry (its grid values and run_evaluate_episodes' record over its
-    envs, taken as run_evaluate_episodes takes it) and a summary line; returns those records."""
+    """--eval 1 --terrain_grid 1 of train, pretrain and bctrain: evaluate_settings on every geometry of terrain_grid(--task_mode), in one
+    terrain-atlas env with env_cfg's configuration and the --dynamic_param dynamics.  A geometry's record leads with its grid values; the
+    summary gives the number of geometries, the mean return over them, and the worst geometry and its return."""
     geoms = terrain_grid(args.task_mode)
     tiles, x0, y0, cell = make_terrain_tiles(args.task_mode, geoms, args.step_y)
     n, G = args.eval_envs, len(geoms)
     env = make_eval_env(args, dict(env_cfg, heightfield=(tiles[0], x0, y0, cell)), n * G)
     env.set_terrain_tiles(tiles, np.repeat(np.arange(G, dtype=np.int32), n))
     del tiles
-    r = run_evaluate_episodes(env, w, b, policy=policy, act_bound=act_bound, max_step=max_step, x_offset=None if x_offset is None else np.tile(x_offset, G))
-    pe = r["per_env"]
-    cols = [pe["return"], pe["length"], pe["success_rate"]] + [pe["terms"][k] for k in EVAL_TERMS]
-    means = torch.stack([torch.stack([c[g * n:(g + 1) * n].double().mean() for c in cols]) for g in range(G)]).tolist()
-    env.close()
-    recs = []
-    for geom, m in zip(geoms, means):
-        rec = dict(geom, mean_return=m[0], mean_length=m[1], success_rate=m[2], terms={k: m[3 + j] for j, k in enumerate(EVAL_TERMS)})
-        recs.append(rec)
-        print(json.dumps(rec), flush=True)
-    worst = min(range(G), key=lambda g: recs[g]["mean_return"])
-    summary = {"geometries": G, "eval_envs": n, "task_mode": args.task_mode, "mean_return": float(np.mean([rc["mean_return"] for rc in recs])),
-               "worst": geoms[worst], "worst_return": recs[worst]["mean_return"]}
-    print(json.dumps(summary), flush=True)
-    return recs + [summary]
+
+    def summary(recs):
+        worst = min(range(G), key=lambda g: recs[g]["mean_return"])
+        return {"geometries": G, "eval_envs": n, "task_mode": args.task_mode, "mean_return": float(np.mean([rc["mean_return"] for rc in recs])),
+                "worst": geoms[worst], "worst_return": recs[worst]["mean_return"]}
+    return evaluate_settings(env, geoms, summary, w, b, policy=policy, act_bound=act_bound, max_step=max_step, x_offset=x_offset)
+
+
+def check_dynamics_grid(p, args):
+    """The argument errors of --dynamics_grid 1 (train, pretrain, bctrain), raised (p.error) before any device work."""
+    if not getattr(args, "dynamics_grid", 0):
+        return
+    if not args.eval:
+        p.error("--dynamics_grid 1 scores a checkpoint or gait on every setting of the dynamics sweep: it needs --eval 1")
+    if getattr(args, "terrain_grid", 0):
+        p.error("--dynamics_grid 1 with --terrain_grid 1: one grid evaluation at a time (each runs one setting per group of envs)")
+    if args.render_dir:
+        p.error("--dynamics_grid 1 with --render_dir: the frames show env 0, and a grid evaluation steps one setting per group of envs")
+
+
+def evaluate_dynamics_grid(args, env_cfg, w, b, policy=None, act_bound=0.3, max_step=EVAL_MAX_STEP, x_offset=None):
+    """--eval 1 --dynamics_grid 1 of train, pretrain and bctrain: evaluate_settings on the 82 settings of dynamics_grid.settings(), in one
+    env with env_cfg's configuration (the --task_mode terrain) whose rows come from one set_dynamics call: env s * eval_envs + j has the
+    run's --dynamic_param (or nominal) row with setting s's group at its level.  A setting's record leads with its group, level and the
+    group's engine values; the summary gives the centre's return and, per group, the worst level, its return and the range of the
+    return over the levels, most sensitive group first."""
+    rows = dynamics_grid.swept_rows(dynamic_param_row(args.dynamic_param))
+    n = args.eval_envs
+    env = VecQuadrupedalEnv(n * len(rows), auto_reset=False, **env_cfg)
+    env.set_dynamics(np.repeat(rows, n, 0))
+
+    def summary(recs):
+        return {"settings": len(recs), "eval_envs": n, "task_mode": args.task_mode, "dynamic_param": args.dynamic_param or None,
+                "centre_return": recs[0]["mean_return"], "groups": dynamics_grid.group_summary(recs[1:], "mean_return")}
+    return evaluate_settings(env, dynamics_grid.setting_records(), summary, w, b, policy=policy, act_bound=act_bound, max_step=max_step,
+                             x_offset=x_offset)
 
 
 def frame_writer(env, args):
@@ -646,15 +693,16 @@ def frame_writer(env, args):
 
 def evaluate(args, env_cfg, act_bound):
     """--eval 1: one deterministic episode per env of the restored agent and ETG (w, b) on the training env's config, at most
-    EVAL_MAX_STEP + 1 control steps (run_evaluate_episodes).  Prints and returns one JSON record; with --terrain_grid 1, the records of
-    evaluate_terrain_grid."""
+    EVAL_MAX_STEP + 1 control steps (run_evaluate_episodes).  Prints and returns one JSON record; with --terrain_grid 1 or
+    --dynamics_grid 1, the records of evaluate_terrain_grid or evaluate_dynamics_grid."""
     n = args.eval_envs
     z = np.load(args.load[:-3] + ".npz")                                                                                      # train.py:439-441
     w, b = z["w"], z["b"]
-    if args.terrain_grid:
+    if args.terrain_grid or getattr(args, "dynamics_grid", 0):
         agent = MujocoAgent(obs_width(args), 12, seed=args.seed)
         agent.restore(args.load)
-        return evaluate_terrain_grid(args, env_cfg, w, b, policy=lambda o, s: agent.predict_batch(o), act_bound=act_bound, max_step=EVAL_MAX_STEP)
+        grid = evaluate_terrain_grid if args.terrain_grid else evaluate_dynamics_grid
+        return grid(args, env_cfg, w, b, policy=lambda o, s: agent.predict_batch(o), act_bound=act_bound, max_step=EVAL_MAX_STEP)
     env = make_eval_env(args, env_cfg, n)
     agent = MujocoAgent(env.observation_dim, 12, seed=args.seed)
     agent.restore(args.load)
